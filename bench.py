@@ -1,10 +1,10 @@
 #!/usr/bin/env python
-"""bench.py — Taylor-score UNet fwd+bwd passes/sec (BASELINE.json metric) on N B200s.
+"""bench.py — Taylor-score UNet fwd+bwd passes/sec (BASELINE.json metric) on N H100s.
 
 A "step" = one pass of ddpm_prune.py:97-102 (add_noise -> UNet fwd -> mse -> full bwd, gradients accumulated) over one synthetic
 Gaussian batch.  Workloads (--config):
   c1 (default)  CIFAR-10 DDPM UNet (tools/ddpm_cifar10_config.json, seed-0 random init), batch 128 x 3x32x32 — BASELINE configs[1]
-                ("DDPM CIFAR-10 32x32 ... 1xB200"; batch from scripts/prune_ddpm_cifar10.sh).
+                (DDPM CIFAR-10 32x32 on one GPU; batch from scripts/prune_ddpm_cifar10.sh).
   c3            google/ddpm-ema-bedroom-256 architecture (seed-0 random init), batch 4 x 3x256x256, ratio 0.05 — BASELINE configs[2]
                 (README.md:140-148), the configuration the north star shards over 8 GPUs.
 Multi-GPU: timesteps are sharded across ranks (weak scaling: every rank runs K steps on its own timesteps) and the flat gradient arena
@@ -12,6 +12,8 @@ is all-reduced ONCE at the end, inside the timed region.  Secondary leg (`finetu
 ddpm_train.py:437-469 on the ratio-0.3 network (imgs/s; fp32-grade and, separately, the bf16 tier of BASELINE configs[3]).
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config c1|c3] [--batch B] [--no-graph]
+                  [--dump-outputs DIR]
+--dump-outputs DIR: what the last timed step returned (dump_outputs); inputs are seeded, so two builds compare output for output.
 Under torchrun the usual RANK/LOCAL_RANK/WORLD_SIZE/MASTER_* env is used; rank 0 prints ONE JSON line.
 """
 import argparse
@@ -71,15 +73,16 @@ def make_model(cfg_key):
 
 
 def peaks():
+    """(HBM GB/s, sustained / burst bf16 TFLOP/s, source); without MEASURED_PEAKS.json the H100 SXM data sheet (700 W), not reached rates."""
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return d.get("hbm_gbs", 6650.0), d.get("bf16_tflops_sustained", 1400.0), d.get("bf16_tflops", 1590.0), "measured"
-    return 6650.0, 1400.0, 1590.0, "fallback"
+        return d.get("hbm_gbs", 3350.0), d.get("bf16_tflops_sustained", 989.0), d.get("bf16_tflops", 989.0), "measured"
+    return 3350.0, 989.0, 989.0, "H100 SXM data sheet"
 
 
 class ClockSampler:
-    """nvidia-smi clocks/throttle sampling DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks/throttle sampling DURING the timed region."""
     Q = ("clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -120,6 +123,22 @@ class ClockSampler:
                 "reasons": sorted(reasons), "samples": len(sm)}
 
 
+DUMP_GRAD_ELEMS = 8 << 20      # gradient elements --dump-outputs writes at most (32 MB of float32)
+
+
+def dump_outputs(out_dir, sc):
+    """The loss, eps_hat (NCHW) and the gradients accumulated so far (all of the flat arena up to DUMP_GRAD_ELEMS elements, else a fixed
+    seeded sample of it) as float32 out_dir/<name>.npy."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    g = sc.plan.grad_arena.reshape(-1)
+    if g.numel() > DUMP_GRAD_ELEMS:
+        idx = torch.randint(g.numel(), (DUMP_GRAD_ELEMS,), generator=torch.Generator().manual_seed(1234)).sort().values
+        g = g[idx.to(g.device)]
+    for name, t in (("loss", sc.loss), ("eps_hat", sc.plan.output_nchw()), ("grads", g)):
+        np.save(os.path.join(out_dir, name + ".npy"), t.detach().float().cpu().numpy())
+
+
 def synth_batch(B, hw=32, seed_off=0):
     g1, g2 = torch.Generator().manual_seed(1 + seed_off), torch.Generator().manual_seed(2 + seed_off)
     return torch.randn(B, 3, hw, hw, generator=g1), torch.randn(B, 3, hw, hw, generator=g2)
@@ -127,7 +146,7 @@ def synth_batch(B, hw=32, seed_off=0):
 
 # ------------------------------------------------------------------------------------------------------------------------
 # baselines: the oracle port (torch ATen ops = the reference's own backend) on the host cores, and the same modules torch-eager
-# on the GPU (cuDNN, TF32 on/off) — SURVEY.md §8(d): "time torch-eager on the same B200 as the real bar to beat"
+# on the GPU (cuDNN, TF32 on/off) — SURVEY.md §8(d): torch-eager on the same GPU is the real bar to beat
 # ------------------------------------------------------------------------------------------------------------------------
 def _oracle_setup(cfg_key, sample_B, sample_hw, device="cpu"):
     model, mcfg, extra = make_model(cfg_key)
@@ -224,7 +243,7 @@ def gpu_eager_passes(cfg_key, B, dev, n=5):
         out["error"] = f"{type(e).__name__}: {str(e)[:160]}"
     finally:
         torch.backends.cudnn.allow_tf32 = prev
-    out["what"] = (f"oracle port (torch functional ops = the reference's ATen/cuDNN path) on the same B200, batch {B} x {c['hw']}x{c['hw']}, "
+    out["what"] = (f"oracle port (torch functional ops = the reference's ATen/cuDNN path) on the same GPU, batch {B} x {c['hw']}x{c['hw']}, "
                    f"CUDA events over {n} passes after 3 warm-ups; cudnn_tf32 = torch default (conv in TF32), fp32 = cudnn.allow_tf32 False")
     torch.cuda.empty_cache()
     return out
@@ -549,6 +568,8 @@ def run_ours(args, rank, world, local_rank):
     barrier()
     clocks = sampler.stop() if rank == 0 else None
     ms = e0.elapsed_time(e1)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, sc)
     eager_launches = lib.dp_launch_count() - c_before
     gpu_launches = eager_launches if args.no_graph else launches_per_pass * args.steps
     # ---------------- end-to-end through host buffers (H2D batch each step, D2H loss each step)
@@ -632,24 +653,17 @@ def run_ours(args, rank, world, local_rank):
     achieved = flops / conv_s / 1e12
     tc = bool(lib.dp_tc_available())
     tf32 = measure_tf32_peak(dev)
-    traffic = None
-    tp = os.path.join(ROOT, "profiles", "r02_conv_traffic.json" if os.path.exists(os.path.join(ROOT, "profiles", "r02_conv_traffic.json"))
-                      else "r01_conv_traffic.json")
-    if os.path.exists(tp) and B == 128 and args.config == "c1":   # dram__bytes_read+write summed over the conv launches of one pass (committed ncu capture)
-        tj = json.load(open(tp))
-        traffic = tj["dram_read_bytes"] + tj["dram_write_bytes"]
-    tier_ceiling = tf_sus / 3.0      # 3 kind::f16 tensor instructions per product (fp16 runs at the bf16 rate MEASURED_PEAKS.json holds)
+    tier_ceiling = tf_sus / 3.0      # 3 fp16 wgmma per product (fp16 runs at the bf16 rate)
     roofline = {"bound": "tensor", "achieved": achieved, "peak": tf_sus, "unit": "TFLOP/s", "frac": achieved / tf_sus,
-                "traffic": traffic, "breakdown_ms": conv_by_tag, "top_layers_ms": conv_by_layer,
+                "breakdown_ms": conv_by_tag, "top_layers_ms": conv_by_layer,
                 "other_launches_ms": other_ms, "tf32_peak_measured": tf32, "tier_ceiling_tflops": tier_ceiling, "frac_of_tier_ceiling": achieved / tier_ceiling,
                 "plan_conv_gflop_per_image": 6.0 * plan_macs / plan_B / 1e9, "plan_linear_gflop_per_image": 6.0 * plan_lin_macs / plan_B / 1e9,
                 "kernel": "conv implicit GEMM (fprop+dgrad+wgrad launches of one pass: %d)" % n_conv,
                 "note": (f"algorithmic conv FLOPs/pass = {B} x {c['conv_flop'] / 1e9:.2f} GFLOP (SURVEY.md §8d) / summed conv-launch device time "
                          f"{conv_s * 1e3:.2f} ms of a {ms / args.steps:.2f} ms step; peak = bf16_tflops_sustained ({which}); "
-                         "fp32-grade tier: " + ("tcgen05 kind::f16 on a 3-product fp16 hi/lo split of power-of-two-scaled operands (22 bits per operand, fp32 accumulation: "
+                         "fp32-grade tier: " + ("fp16 wgmma on a 3-product fp16 hi/lo split of power-of-two-scaled operands (22 bits per operand, fp32 accumulation: "
                                                  "tier ceiling = peak / 3; tf32_peak_measured = cuBLAS TF32, the rate torch-eager's cuDNN default runs at)" if tc
-                                                 else "CUDA-core FFMA (SIMT) — tensor path not active") +
-                         "; traffic = DRAM bytes of all conv launches of one pass (committed ncu capture, C1 only)")}
+                                                 else "CUDA-core FFMA (SIMT) — tensor path not active"))}
     value = world * args.steps / (ms * 1e-3)
     e2e = world * args.steps / (ms_e2e * 1e-3)
     cpu = cpu_oracle_passes(args.config, B, min_seconds=12.0, max_passes=8) if args.gpus == 1 and not args.no_cpu else None
@@ -660,7 +674,7 @@ def run_ours(args, rank, world, local_rank):
         "dtype": "f32", "data": "synthetic",
         "config": {"workload": f"{c['name']} Taylor pass, batch {B} x 3x{hw}x{hw} per GPU, "
                                f"timesteps sharded over {world} GPU(s), one grad all-reduce at the end",
-                   "l2": f"per-pass working set (activations+grads, {plan_bytes / 2**30:.1f} GiB) >> 126 MB L2: inputs larger than L2, no explicit flush",
+                   "l2": f"per-pass working set (activations+grads, {plan_bytes / 2**30:.1f} GiB) >> 50 MB L2: inputs larger than L2, no explicit flush",
                    "cuda_graph": not args.no_graph, "imgs_per_s": value * B},
         "clocks": clocks, "gpu_launches": int(gpu_launches),
         "e2e": {"value": e2e, "unit": UNIT, "h2d_bytes_per_step": int(2 * clean.numel() * 4 + 8 * B), "d2h_bytes_per_step": 4,
@@ -695,6 +709,8 @@ def main():
     ap.add_argument("--profile-pass", action="store_true", help="run one eager pass inside cudaProfilerStart/Stop (ncu)")
     ap.add_argument("--no-finetune", action="store_true", help="skip the secondary finetune imgs/s legs")
     ap.add_argument("--no-c3", action="store_true", help="skip the secondary BASELINE-config-3 (LSUN-256) scoring leg of the default run")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the loss, eps_hat and (a seeded sample of) the gradients as DIR/<name>.npy")
     args = ap.parse_args()
     if args.batch is None:
         args.batch = CONFIGS[args.config]["batch"]

@@ -1,4 +1,4 @@
-"""diff_pruning_b200 — B200-native Taylor-importance / finetune hot path of VainF/Diff-Pruning.
+"""diff_pruning_b200 — H100-native (sm_90a) Taylor-importance / finetune hot path of VainF/Diff-Pruning.
 
 See DESIGN.md. Public surface mirrors the reference's (SURVEY.md §8(b1)).
 """

@@ -137,7 +137,7 @@ def load():
     if not os.path.exists(path):
         raise DpError(
             f"diff_pruning_b200: {LIB_PATH} not found. Build it with `python -c 'import __graft_entry__ as g; "
-            "g.build()'` (nvcc, sm_100a). There is no CPU / PyTorch fallback for the hot path.")
+            "g.build()'` (nvcc, sm_90a). There is no CPU / PyTorch fallback for the hot path.")
     lib = C.CDLL(path)
     for name, (res, args) in _SIGS.items():
         fn = getattr(lib, name)

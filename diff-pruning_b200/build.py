@@ -1,4 +1,4 @@
-"""Build libdpb200.so in-tree with nvcc for sm_100a (no torch extension machinery: the library is a plain
+"""Build libdpb200.so in-tree with nvcc for sm_90a (H100) (no torch extension machinery: the library is a plain
 C-ABI shared object, loaded with ctypes)."""
 import os
 import subprocess
@@ -30,7 +30,7 @@ def build(force=False, verbose=False):
     for s in srcs:
         o = s[:-3] + ".o"
         if force or _newer([s] + [d for d in deps if not d.endswith(".cu")], o):
-            cmd = [nvcc, "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+            cmd = [nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
                    "-Xcompiler", "-fPIC", "-I", os.path.join(ROOT, "include"), "-I", CSRC, "-c", s, "-o", o]
             if have_tc:
                 cmd.insert(1, "-DDPB200_HAVE_TC")

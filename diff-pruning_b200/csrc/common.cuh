@@ -1,10 +1,12 @@
-// common.cuh — shared helpers for libdpb200 (sm_100a only).
+// common.cuh — shared helpers for libdpb200 (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include "dpb200.h"
 
 extern int g_dp_last_cuda_error;
+// grid-stride kernels cap their grids at a multiple of the SM count (H100 SXM: 132)
+constexpr int DP_NUM_SMS = 132;
 extern long long g_dp_launch_count;
 
 static inline int dp_check_launch() {

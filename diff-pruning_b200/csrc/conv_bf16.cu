@@ -1,4 +1,4 @@
-// conv_bf16.cu — the single-pass tensor tier: tcgen05.mma kind::f16 on BF16 operands, fp32 accumulation in TMEM.
+// conv_bf16.cu — the single-pass tensor tier: wgmma on BF16 operands, fp32 accumulation in registers.
 //
 // What it is for: the pruned-UNet finetune step under `--mixed_precision bf16` (ddpm_train.py:200-208,255-261: torch.autocast runs
 // conv2d / linear in bf16, GroupNorm / softmax / loss / Adam / EMA in fp32) — BASELINE configs[3].  Operands are rounded to bf16 (RNE)
@@ -6,27 +6,27 @@
 // in the tensor core and accumulate in fp32; outputs, the residual stream and all gradients stay fp32.
 //
 // Unlike the fp32-grade split kernels (conv_tc.cu) nothing has to touch the operands between TMA and the MMA: TMA -> swizzled shared memory ->
-// tcgen05.mma, no splitter warps, no proxy fence in the loop.  One pipeline stage = 64 bf16 of GEMM-K = one 128-byte swizzle row.
+// wgmma, no splitting, no proxy fence in the loop.  One pipeline stage = 64 bf16 of GEMM-K = one 128-byte swizzle row.  Warpgroup roles:
+// sm90.cuh (TMA producer + two consumer warpgroups of 64 tile rows each).
 //   conv_bf16_kernel   fprop / dgrad (stride-1 dgrad = tap-flipped fprop; stride 2 through TMA element strides / parity classes):
 //                      persistent, 1 CTA per SM, tile 128 pixels x up to 256 output channels (one N tile covers every layer of the
-//                      DDPM configs up to 256 channels, so the activation tile is fetched once), two TMEM accumulator sets so the
-//                      epilogue of tile i overlaps the main loop of tile i+1.  A 128x256x64 stage is 48 KB of operands for 536 tensor
-//                      clocks = 90 B/clk — the L2->SM path (~60 B/clk/SM), not the tensor pipe, bounds this kernel; that is why the N
-//                      tile is as wide as TMEM allows.
+//                      DDPM configs up to 256 channels, so the activation tile is fetched once).
 //   wgrad_bf16_kernel  dW[k][tap][c] = sum_pix dy[pix][k] x[pix@tap][c]: both operands MN-major (pixel-major activations) straight
 //                      from TMA (SWIZZLE_128B, 64 channels x 64 pixels per box), tile 128 out-channels x up to 256 in-channels,
 //                      split-K over pixels into the fp32 workspace that dp_conv2d_wgrad_reduce sums in fixed order.
+// Both are instantiated per N tile width (64, 128, 192, 256): wgmma takes N as an immediate and the accumulators live in registers.
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <mutex>
 #include "common.cuh"
+#include "sm90.cuh"
 
 namespace {
+using namespace sm90;
 
-constexpr int BM = 128;            // GEMM-M tile: 128 output pixels = TMEM lanes
+constexpr int BM = 128;            // GEMM-M tile: 128 output pixels (64 per consumer warpgroup)
 constexpr int KB = 64;             // bf16 elements of GEMM-K per pipeline stage (one 128-byte swizzle row)
 constexpr int A_BYTES = BM * KB * 2;   // 16 KB
-constexpr int NTHREADS = 192;      // warp 0 TMA producer | warp 1 MMA issuer | warps 2-5 epilogue
 constexpr int MAX_SMEM = 227 * 1024;
 
 struct BfParams {
@@ -42,8 +42,7 @@ struct BfParams {
   signed char dh[9], dw[9], wt[9];
   int os, oa, ob, Ho, Wo;      // output pixel = (p*os + oa, q*os + ob) on an [Ho][Wo] grid
   int in_stride;
-  int bn_tile;                 // N tile width = rows of the weight box (multiple of 16, <= 256)
-  int stages, stage_bytes;
+  int stages;
 };
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -80,84 +79,30 @@ __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* map
       ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
 }
-// K-major, 128B-swizzled operand tile (cute::UMMA::SmemDescriptor): start>>4 | LBO(1)<<16 | SBO(1024 B >> 4)<<32 | version 1 << 46 |
-// SWIZZLE_128B (2) << 61.  Rows are 128 bytes (64 bf16), 8-row groups are 1024 B apart.
-__device__ __forceinline__ uint64_t desc_k(uint32_t saddr) {
-  return (uint64_t)((saddr & 0x3FFFF) >> 4) | (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
-}
-// MN-major, 128B-swizzled operand tile (canonical ((8,n),(8,k)):((1,LBO),(8,SBO)) in 16-byte units, mma_traits_sm100.hpp): a block of
-// 64 channels x P pixels = P rows of 128 bytes; 8-pixel K groups are SBO = 1024 B apart, 64-channel blocks LBO = lbo bytes apart.
-__device__ __forceinline__ uint64_t desc_mn(uint32_t saddr, uint32_t lbo_bytes) {
-  return (uint64_t)((saddr & 0x3FFFF) >> 4) | ((uint64_t)(lbo_bytes >> 4) << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
-}
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t acc) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(acc)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile("{\n\t.reg .pred P1;\n\telect.sync _|P1, 0xffffffff;\n\tselp.u32 %0, 1, 0, P1;\n\t}" : "=r"(pred));
-  return pred != 0;
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-        "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-        "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// instruction descriptor (cute::UMMA::InstrDescriptor): D = F32 (1 << 4) | A = BF16 (1 << 7) | B = BF16 (1 << 10) | a_major bit 15 |
-// b_major bit 16 | N >> 3 at bit 17 | M >> 4 at bit 24
-__device__ __forceinline__ uint32_t idesc_bf16(uint32_t n, bool mn_major) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (mn_major ? ((1u << 15) | (1u << 16)) : 0u) | ((n >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
-}
-
 // ------------------------------------------------------------------------------------------------ fprop / dgrad
-__global__ void __launch_bounds__(NTHREADS, 1)
+// NB = N tile / 64 = rows of the weight box / 64
+template <int NB>
+__global__ void __launch_bounds__(THREADS, 1)
 conv_bf16_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB, const BfParams p,
                  const int tiles_m, const int total_tiles) {
+  constexpr int BNT = 64 * NB;
+  constexpr int B_BYTES = BNT * 128;
+  constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t pad_to = ((raw + 1023u) & ~1023u) - raw;   // SWIZZLE_128B needs 1024-byte aligned tiles
-  uint8_t* smem = smem_raw + pad_to;
   const uint32_t sbase = raw + pad_to;
   const int S = p.stages;
-  const uint32_t bar0 = sbase + (uint32_t)(S * p.stage_bytes);
+  const uint32_t bar0 = sbase + (uint32_t)(S * STAGE_BYTES);
   auto full_bar = [&](int s) { return bar0 + 8u * s; };
   auto empty_bar = [&](int s) { return bar0 + 8u * (S + s); };
-  auto tfull_bar = [&](int b) { return bar0 + 8u * (2 * S + b); };
-  auto tempty_bar = [&](int b) { return bar0 + 8u * (2 * S + 2 + b); };
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + S * p.stage_bytes + 8 * (2 * S + 4));
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7, tid = threadIdx.x & 127;
   if (threadIdx.x == 0) {
-    for (int s = 0; s < S; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 1); }
-    for (int b = 0; b < 2; ++b) { mbar_init(tfull_bar(b), 1); mbar_init(tempty_bar(b), 128); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    for (int s = 0; s < S; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 8); }   // one arrival per consumer warp
+    mbar_init_fence();
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(512) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_slot;
   const int iters_per_tile = p.ntaps * p.kchunks;
-  const int BNT = p.bn_tile;
-  const uint32_t b_bytes = (uint32_t)BNT * 128u;
 
   auto tile_coords = [&](int tile, int& q0, int& p0, int& n0, int& nblk) {
     nblk = tile / tiles_m;
@@ -168,116 +113,90 @@ conv_bf16_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant
     q0 = tw * p.bw; p0 = th * p.bh; n0 = tn * p.bn;
   };
 
-  if (warp == 0) {
-    if (elect_one()) {
-      asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&mapA)) : "memory");
-      asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&mapB)) : "memory");
+  if (wg == 0) {
+    setmaxnreg_dec<40>();
+    if (threadIdx.x == 0) {
+      prefetch_map(&mapA); prefetch_map(&mapB);
       int s = 0; uint32_t ph = 0;
       for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
         int q0, p0, n0, nblk;
         tile_coords(tile, q0, p0, n0, nblk);
         for (int it = 0; it < iters_per_tile; ++it) {
           mbar_wait(empty_bar(s), ph ^ 1u);
-          mbar_expect_tx(full_bar(s), A_BYTES + b_bytes);
+          mbar_expect_tx(full_bar(s), STAGE_BYTES);
           const int tap = it / p.kchunks, kc = it - tap * p.kchunks;
-          const uint32_t st = sbase + (uint32_t)(s * p.stage_bytes);
+          const uint32_t st = sbase + (uint32_t)(s * STAGE_BYTES);
           tma_load_4d(st, &mapA, full_bar(s), kc * KB, q0 * p.in_stride + p.dw[tap], p0 * p.in_stride + p.dh[tap], n0);
           tma_load_3d(st + A_BYTES, &mapB, full_bar(s), kc * KB, nblk * BNT, p.wt[tap]);
           if (++s == S) { s = 0; ph ^= 1u; }
         }
       }
     }
-    __syncwarp();
-  } else if (warp == 1) {
-    int s = 0; uint32_t ph = 0, tl = 0;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++tl) {
-      const int nblk = tile / tiles_m;
-      const int n_valid = min(BNT, p.Nout - nblk * BNT);
-      const uint32_t idesc = idesc_bf16((uint32_t)((n_valid + 15) & ~15), false);
-      const uint32_t b = tl & 1u, use = tl >> 1;
-      mbar_wait(tempty_bar(b), (use & 1u) ^ 1u);          // epilogue has drained this accumulator set
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const uint32_t acc = tmem_base + b * 256u;
-      for (int it = 0; it < iters_per_tile; ++it) {
-        mbar_wait(full_bar(s), ph);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t st = sbase + (uint32_t)(s * p.stage_bytes);
-        if (elect_one()) {
+    return;
+  }
+  setmaxnreg_inc<232>();
+  const int c = wg - 1;                       // consumer warpgroup: tile rows 64c .. 64c + 63
+  const int warp = tid >> 5, lane = tid & 31;
+  int s = 0; uint32_t ph = 0;
+  for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+    float acc[BNT / 2];
+    int prev_s = 0;
+    for (int it = 0; it < iters_per_tile; ++it) {
+      mbar_wait(full_bar(s), ph);
+      const uint32_t st = sbase + (uint32_t)(s * STAGE_BYTES);
+      wgmma_fence();
 #pragma unroll
-          for (int k = 0; k < KB / 16; ++k)     // UMMA K = 16 bf16 = 32 bytes inside the 128-byte swizzle row
-            umma_bf16(acc, desc_k(st + k * 32), desc_k(st + A_BYTES + k * 32), idesc, (it > 0 || k > 0) ? 1u : 0u);
-          umma_commit(empty_bar(s));            // the stage is free once these MMAs have read it
-          if (it == iters_per_tile - 1) umma_commit(tfull_bar(b));
-        }
-        __syncwarp();
-        if (++s == S) { s = 0; ph ^= 1u; }
-      }
+      for (int k = 0; k < KB / 16; ++k)     // wgmma K = 16 bf16 = 32 bytes inside the 128-byte swizzle row
+        wgmma_bf16<BNT, 0, 0>(acc, desc_k(st + c * 8192 + k * 32), desc_k(st + A_BYTES + k * 32), (it > 0 || k > 0) ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<1>();                      // the previous stage's MMAs have read their operands: hand it back to TMA
+      if (it > 0 && lane == 0) mbar_arrive(empty_bar(prev_s));
+      prev_s = s;
+      if (++s == S) { s = 0; ph ^= 1u; }
     }
-  } else {
-    // ---- epilogue warps 2..5 (TMEM lane quarter = warp & 3)
-    const int q = warp & 3;
-    const int row = q * 32 + lane;
-    const uint32_t lane_addr = (uint32_t)(q * 32) << 16;
-    const int w_l = row % p.bw, h_l = (row / p.bw) % p.bh, n_l = row / (p.bw * p.bh);
-    uint32_t tl = 0;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++tl) {
-      int q0, p0, n0, nblk;
-      tile_coords(tile, q0, p0, n0, nblk);
-      const uint32_t b = tl & 1u, use = tl >> 1;
-      mbar_wait(tfull_bar(b), use & 1u);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+    wgmma_wait<0>();
+    fence_regs(acc);
+    if (lane == 0) mbar_arrive(empty_bar(prev_s));
+
+    int q0, p0, n0, nblk;
+    tile_coords(tile, q0, p0, n0, nblk);
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const int row = 64 * c + 16 * warp + (lane >> 2) + 8 * i;
+      const int w_l = row % p.bw, h_l = (row / p.bw) % p.bh, n_l = row / (p.bw * p.bh);
       const int img = n0 + n_l;
-      const bool row_ok = img < p.Nimg;
+      if (img >= p.Nimg) continue;
       const long long m = ((long long)img * p.Ho + ((p0 + h_l) * p.os + p.oa)) * p.Wo + ((q0 + w_l) * p.os + p.ob);
       float* yrow = p.y + m * p.ldy;
       const float* rrow = p.residual ? p.residual + m * p.ld_res : nullptr;
       const float* arow = p.rowadd ? p.rowadd + (long long)img * p.ld_rowadd : nullptr;
-      const int n_valid = min(BNT, p.Nout - nblk * BNT);
-      const int nchunks = (n_valid + 31) >> 5;
-#pragma unroll 1
-      for (int j = 0; j < nchunks; ++j) {
-        uint32_t v[32];
-        tmem_ld32(tmem_base + lane_addr + b * 256u + (uint32_t)(j * 32), v);
-        if (j == nchunks - 1) {   // the accumulator is in registers: hand the TMEM set back to the MMA warp
-          asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-          mbar_arrive(tempty_bar(b));
-        }
-        if (row_ok) {
-          const int c0 = nblk * BNT + j * 32;
-          if (p.vec4 && c0 + 32 <= p.Nout) {
 #pragma unroll
-            for (int i = 0; i < 32; i += 4) {
-              float4 o = make_float4(__uint_as_float(v[i]), __uint_as_float(v[i + 1]), __uint_as_float(v[i + 2]), __uint_as_float(v[i + 3]));
-              if (p.bias) { float4 t = __ldg(reinterpret_cast<const float4*>(p.bias + c0 + i)); o.x += t.x; o.y += t.y; o.z += t.z; o.w += t.w; }
-              if (arow) { float4 t = __ldg(reinterpret_cast<const float4*>(arow + c0 + i)); o.x += t.x; o.y += t.y; o.z += t.z; o.w += t.w; }
-              if (rrow) { float4 t = __ldg(reinterpret_cast<const float4*>(rrow + c0 + i)); o.x += t.x; o.y += t.y; o.z += t.z; o.w += t.w; }
-              float4* dst = reinterpret_cast<float4*>(yrow + c0 + i);
-              if (p.accumulate) { float4 t = *dst; o.x += t.x; o.y += t.y; o.z += t.z; o.w += t.w; }
-              *dst = o;
-            }
-          } else {
+      for (int j = 0; j < BNT / 8; ++j) {
+        const int col = nblk * BNT + 8 * j + 2 * (lane & 3);
+        float o[2] = {acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]};
+        if (p.vec4 && col + 2 <= p.Nout) {
+          if (p.bias) { const float2 t = __ldg(reinterpret_cast<const float2*>(p.bias + col)); o[0] += t.x; o[1] += t.y; }
+          if (arow) { const float2 t = __ldg(reinterpret_cast<const float2*>(arow + col)); o[0] += t.x; o[1] += t.y; }
+          if (rrow) { const float2 t = __ldg(reinterpret_cast<const float2*>(rrow + col)); o[0] += t.x; o[1] += t.y; }
+          float2* dst = reinterpret_cast<float2*>(yrow + col);
+          if (p.accumulate) { const float2 t = *dst; o[0] += t.x; o[1] += t.y; }
+          *dst = make_float2(o[0], o[1]);
+        } else {
 #pragma unroll
-            for (int i = 0; i < 32; ++i) {
-              const int c = c0 + i;
-              if (c < p.Nout) {
-                float o = __uint_as_float(v[i]);
-                if (p.bias) o += __ldg(p.bias + c);
-                if (arow) o += __ldg(arow + c);
-                if (rrow) o += __ldg(rrow + c);
-                if (p.accumulate) o += yrow[c];
-                yrow[c] = o;
-              }
+          for (int e = 0; e < 2; ++e) {
+            const int cc = col + e;
+            if (cc < p.Nout) {
+              float ov = o[e];
+              if (p.bias) ov += __ldg(p.bias + cc);
+              if (arow) ov += __ldg(arow + cc);
+              if (rrow) ov += __ldg(rrow + cc);
+              if (p.accumulate) ov += yrow[cc];
+              yrow[cc] = ov;
             }
           }
         }
       }
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  }
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512) : "memory");
   }
 }
 
@@ -287,42 +206,34 @@ struct WgBfParams {
   int R, S, pad;
   int bw, bh, bn, tiles_w, tiles_h;   // 64-pixel box of the dy grid
   int total_chunks, chunks_per_split;
-  int c_tiles, ct_width;         // in-channel tiles of ct_width (multiple of 64, <= 256)
+  int c_tiles, ct_width;         // in-channel tiles of ct_width (= 64 * NB)
   float* ws;
   int in_stride;
-  int stages, stage_bytes, x_blocks;   // x_blocks = ct_width / 64
+  int stages;
 };
 constexpr int WG_PIX = 64;                 // pixels (GEMM-K) per stage
 constexpr int BLK_BYTES = WG_PIX * 128;    // one [64 px][64 ch] bf16 block = 8 KB
 
-__global__ void __launch_bounds__(NTHREADS, 1)
+// stage: dy blocks 0,1 (out-channels 0-63, 64-127 of the tile: consumer warpgroup c multiplies block c) | x blocks 0..NB-1
+template <int NB>
+__global__ void __launch_bounds__(THREADS, 1)
 wgrad_bf16_kernel(const __grid_constant__ CUtensorMap mapDy, const __grid_constant__ CUtensorMap mapX, const WgBfParams p) {
-  // stage: dy blocks 0,1 (out-channels 0-63, 64-127 of the tile) | x blocks 0..x_blocks-1
+  constexpr int BNT = 64 * NB;
+  constexpr int STAGE_BYTES = (2 + NB) * BLK_BYTES;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t pad_to = ((raw + 1023u) & ~1023u) - raw;
-  uint8_t* smem = smem_raw + pad_to;
   const uint32_t sbase = raw + pad_to;
   const int S = p.stages;
-  const uint32_t bar0 = sbase + (uint32_t)(S * p.stage_bytes);
+  const uint32_t bar0 = sbase + (uint32_t)(S * STAGE_BYTES);
   auto full_bar = [&](int s) { return bar0 + 8u * s; };
   auto empty_bar = [&](int s) { return bar0 + 8u * (S + s); };
-  const uint32_t tmem_full_bar = bar0 + 8u * (2 * S);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + S * p.stage_bytes + 8 * (2 * S + 1));
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7, tid = threadIdx.x & 127;
   if (threadIdx.x == 0) {
-    for (int s = 0; s < S; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 1); }
-    mbar_init(tmem_full_bar, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    for (int s = 0; s < S; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 8); }
+    mbar_init_fence();
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(256) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_slot;
 
   const int T = p.R * p.S;
   int tile = blockIdx.x;
@@ -333,13 +244,13 @@ wgrad_bf16_kernel(const __grid_constant__ CUtensorMap mapDy, const __grid_consta
   const int chunk0 = blockIdx.y * p.chunks_per_split;
   const int chunk1 = min(p.total_chunks, chunk0 + p.chunks_per_split);
   const int num_iters = max(0, chunk1 - chunk0);
-  const int c_valid = min(p.ct_width, p.C - ct * p.ct_width);
-  const int xb = (c_valid + 63) >> 6;            // 64-channel x blocks that hold valid channels
+  const int c_valid = min(BNT, p.C - ct * BNT);
+  const int xb = (c_valid + 63) >> 6;            // 64-channel x blocks that hold valid channels (the others only feed unstored columns)
 
-  if (warp == 0) {
-    if (elect_one()) {
-      asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&mapDy)) : "memory");
-      asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&mapX)) : "memory");
+  if (wg == 0) {
+    setmaxnreg_dec<40>();
+    if (threadIdx.x == 0) {
+      prefetch_map(&mapDy); prefetch_map(&mapX);
       int s = 0; uint32_t ph = 0;
       for (int it = 0; it < num_iters; ++it) {
         mbar_wait(empty_bar(s), ph ^ 1u);
@@ -349,68 +260,52 @@ wgrad_bf16_kernel(const __grid_constant__ CUtensorMap mapDy, const __grid_consta
         const int th = (chunk / p.tiles_w) % p.tiles_h;
         const int tn = chunk / (p.tiles_w * p.tiles_h);
         const int q0 = tw * p.bw, p0 = th * p.bh, n0 = tn * p.bn;
-        const uint32_t st = sbase + (uint32_t)(s * p.stage_bytes);
+        const uint32_t st = sbase + (uint32_t)(s * STAGE_BYTES);
         tma_load_4d(st, &mapDy, full_bar(s), kt * 128, q0, p0, n0);
         tma_load_4d(st + BLK_BYTES, &mapDy, full_bar(s), kt * 128 + 64, q0, p0, n0);
         for (int b = 0; b < xb; ++b)
-          tma_load_4d(st + (2 + b) * BLK_BYTES, &mapX, full_bar(s), ct * p.ct_width + b * 64, q0 * p.in_stride + sx - p.pad,
+          tma_load_4d(st + (2 + b) * BLK_BYTES, &mapX, full_bar(s), ct * BNT + b * 64, q0 * p.in_stride + sx - p.pad,
                       p0 * p.in_stride + r - p.pad, n0);
         if (++s == S) { s = 0; ph ^= 1u; }
       }
     }
-    __syncwarp();
-  } else if (warp == 1) {
-    const uint32_t idesc = idesc_bf16((uint32_t)((c_valid + 15) & ~15), true);
-    if (num_iters == 0) {   // empty split: release the epilogue (it writes zeros)
-      if (elect_one()) umma_commit(tmem_full_bar);
-      __syncwarp();
-    }
-    int s = 0; uint32_t ph = 0;
-    for (int it = 0; it < num_iters; ++it) {
-      mbar_wait(full_bar(s), ph);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const uint32_t st = sbase + (uint32_t)(s * p.stage_bytes);
-      if (elect_one()) {
-#pragma unroll
-        for (int k = 0; k < WG_PIX / 16; ++k)   // 16 pixels = two 8-pixel K groups = 2048 bytes further into every block
-          umma_bf16(tmem_base, desc_mn(st + k * 2048, BLK_BYTES), desc_mn(st + 2 * BLK_BYTES + k * 2048, BLK_BYTES), idesc,
-                    (it > 0 || k > 0) ? 1u : 0u);
-        umma_commit(empty_bar(s));
-        if (it == num_iters - 1) umma_commit(tmem_full_bar);
-      }
-      __syncwarp();
-      if (++s == S) { s = 0; ph ^= 1u; }
-    }
-  } else {
-    const int q = warp & 3;
-    const uint32_t lane_addr = (uint32_t)(q * 32) << 16;
-    mbar_wait(tmem_full_bar, 0);
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const int kout = kt * 128 + q * 32 + lane;
-    const long long TC_ = (long long)T * p.C;
-    float* wrow = p.ws + ((long long)blockIdx.y * p.K + kout) * TC_ + (long long)tap * p.C + (long long)ct * p.ct_width;
-    const int nchunks = (c_valid + 31) >> 5;
-    if (num_iters == 0) {
-      if (kout < p.K)
-        for (int c = 0; c < c_valid; ++c) wrow[c] = 0.f;
-    } else {
-#pragma unroll 1
-      for (int j = 0; j < nchunks; ++j) {
-        uint32_t v[32];
-        tmem_ld32(tmem_base + lane_addr + (uint32_t)(j * 32), v);
-        if (kout < p.K) {
-#pragma unroll
-          for (int i = 0; i < 32; ++i)
-            if (j * 32 + i < c_valid) wrow[j * 32 + i] = __uint_as_float(v[i]);
-        }
-      }
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+    return;
   }
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(256) : "memory");
+  setmaxnreg_inc<232>();
+  const int c = wg - 1;
+  const int warp = tid >> 5, lane = tid & 31;
+  float acc[BNT / 2];
+  int s = 0, prev_s = 0; uint32_t ph = 0;
+  for (int it = 0; it < num_iters; ++it) {
+    mbar_wait(full_bar(s), ph);
+    const uint32_t st = sbase + (uint32_t)(s * STAGE_BYTES);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < WG_PIX / 16; ++k)   // 16 pixels = two 8-pixel K groups = 2048 bytes further into every block
+      wgmma_bf16<BNT, 1, 1>(acc, desc_mn(st + c * BLK_BYTES + k * 2048, BLK_BYTES), desc_mn(st + 2 * BLK_BYTES + k * 2048, BLK_BYTES),
+                            (it > 0 || k > 0) ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<1>();
+    if (it > 0 && lane == 0) mbar_arrive(empty_bar(prev_s));
+    prev_s = s;
+    if (++s == S) { s = 0; ph ^= 1u; }
+  }
+  wgmma_wait<0>();
+  fence_regs(acc);
+  const long long TC_ = (long long)T * p.C;
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    const int kout = kt * 128 + 64 * c + 16 * warp + (lane >> 2) + 8 * i;
+    if (kout >= p.K) continue;
+    float* wrow = p.ws + ((long long)blockIdx.y * p.K + kout) * TC_ + (long long)tap * p.C + (long long)ct * BNT;
+#pragma unroll
+    for (int j = 0; j < BNT / 8; ++j)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int col = 8 * j + 2 * (lane & 3) + e;
+        // an empty split accumulated nothing (the registers hold garbage): it contributes zeros
+        if (col < c_valid) wrow[col] = num_iters ? acc[4 * j + 2 * i + e] : 0.f;
+      }
   }
 }
 
@@ -462,7 +357,7 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t,
                                   CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 EncodeTiledFn g_encode = nullptr;
 int g_state = -1;
-int g_num_sms = 148;
+int g_num_sms = 132;   // H100 SXM; bf_init reads the device's count
 std::mutex g_mutex;
 
 int bf_init() {
@@ -471,14 +366,17 @@ int bf_init() {
   g_state = 0;
   int dev = 0, major = 0;
   if (cudaGetDevice(&dev) != cudaSuccess) { (void)cudaGetLastError(); return 0; }
-  if (cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev) != cudaSuccess || major != 10) { (void)cudaGetLastError(); return 0; }
+  if (cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev) != cudaSuccess || major != 9) { (void)cudaGetLastError(); return 0; }
   void* fn = nullptr;
   cudaDriverEntryPointQueryResult qres;
   if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres) != cudaSuccess || !fn ||
       qres != cudaDriverEntryPointSuccess) { (void)cudaGetLastError(); return 0; }
   g_encode = (EncodeTiledFn)fn;
-  bool ok = cudaFuncSetAttribute(conv_bf16_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, MAX_SMEM) == cudaSuccess;
-  ok = ok && cudaFuncSetAttribute(wgrad_bf16_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, MAX_SMEM) == cudaSuccess;
+  bool ok = true;
+  for (const void* k : {(const void*)conv_bf16_kernel<1>, (const void*)conv_bf16_kernel<2>, (const void*)conv_bf16_kernel<3>,
+                        (const void*)conv_bf16_kernel<4>, (const void*)wgrad_bf16_kernel<1>, (const void*)wgrad_bf16_kernel<2>,
+                        (const void*)wgrad_bf16_kernel<3>, (const void*)wgrad_bf16_kernel<4>})
+    ok = ok && cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, MAX_SMEM) == cudaSuccess;
   cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev);
   if (!ok) { (void)cudaGetLastError(); return 0; }
   g_state = 1;
@@ -533,9 +431,10 @@ int launch_bf16(const void* act, long long ld_act, int Nimg, int H, int W, int K
   int bw, bh, bn;
   if (!pick_box(BM, H, W, bw, bh, bn)) return DP_ERR_UNSUPPORTED;
   if (bw * in_stride > 256 || bh * in_stride > 256) return DP_ERR_UNSUPPORTED;
-  // N tile: as wide as possible (<= 256) so the activation tile is fetched once; balanced over the tiles it takes
+  // N tile: as wide as possible (<= 256) so the activation tile is fetched once; balanced over the tiles it takes, a multiple of 64
+  // (one instantiation per width)
   const int n_tiles = (Nout + 255) / 256;
-  int bn_tile = ((Nout + n_tiles - 1) / n_tiles + 15) & ~15;
+  int bn_tile = ((Nout + n_tiles - 1) / n_tiles + 63) & ~63;
   if (bn_tile > 256) bn_tile = 256;
   if (dry) return DP_OK;
   CUtensorMap mA, mB;
@@ -564,17 +463,21 @@ int launch_bf16(const void* act, long long ld_act, int Nimg, int H, int W, int K
   p.accumulate = accumulate;
   auto al16 = [](const void* q, long long ld) { return q == nullptr || ((((uintptr_t)q) & 15) == 0 && (ld % 4) == 0); };
   p.vec4 = (al16(out, ld_out) && al16(bias, 0) && al16(rowadd, ld_rowadd) && al16(residual, ld_res)) ? 1 : 0;
-  p.bn_tile = bn_tile;
-  p.stage_bytes = A_BYTES + ((bn_tile * 128 + 1023) & ~1023);     // every tile starts 1024-byte aligned
-  int stages = (MAX_SMEM - 2048) / p.stage_bytes;
+  const int stage_bytes = A_BYTES + bn_tile * 128;     // every tile starts 1024-byte aligned
+  int stages = (MAX_SMEM - 2048) / stage_bytes;
   if (stages > 8) stages = 8;
   if (stages < 2) return DP_ERR_UNSUPPORTED;
   p.stages = stages;
   const int tiles_n = (Nimg + bn - 1) / bn;
   const int tiles_m = p.tiles_w * p.tiles_h * tiles_n, total = tiles_m * n_tiles;
   const int ctas = total < g_num_sms ? total : g_num_sms;
-  const size_t smem = (size_t)stages * p.stage_bytes + 2048;
-  conv_bf16_kernel<<<ctas, NTHREADS, smem, st>>>(mA, mB, p, tiles_m, total);
+  const size_t smem = (size_t)stages * stage_bytes + 2048;
+  switch (bn_tile / 64) {
+    case 1: conv_bf16_kernel<1><<<ctas, THREADS, smem, st>>>(mA, mB, p, tiles_m, total); break;
+    case 2: conv_bf16_kernel<2><<<ctas, THREADS, smem, st>>>(mA, mB, p, tiles_m, total); break;
+    case 3: conv_bf16_kernel<3><<<ctas, THREADS, smem, st>>>(mA, mB, p, tiles_m, total); break;
+    default: conv_bf16_kernel<4><<<ctas, THREADS, smem, st>>>(mA, mB, p, tiles_m, total); break;
+  }
   return dp_check_launch();
 }
 
@@ -655,15 +558,21 @@ int wgrad_impl(const dp_conv_bf16_args* a, cudaStream_t st, int dry) {
   p.chunks_per_split = (p.total_chunks + a->splits - 1) / a->splits;
   p.ct_width = dp_bf16_wgrad_ctile(a->C);
   p.c_tiles = (a->C + p.ct_width - 1) / p.ct_width;
-  p.x_blocks = p.ct_width / 64;
+  const int x_blocks = p.ct_width / 64;
   p.ws = a->workspace;
-  p.stage_bytes = (2 + p.x_blocks) * BLK_BYTES;
-  int stages = (MAX_SMEM - 2048) / p.stage_bytes;
+  const int stage_bytes = (2 + x_blocks) * BLK_BYTES;
+  int stages = (MAX_SMEM - 2048) / stage_bytes;
   if (stages > 8) stages = 8;
   p.stages = stages;
   const int k_tiles = (a->K + 127) / 128;
   dim3 grid((unsigned)(k_tiles * p.c_tiles * a->R * a->S), (unsigned)a->splits);
-  wgrad_bf16_kernel<<<grid, NTHREADS, (size_t)stages * p.stage_bytes + 2048, st>>>(mDy, mX, p);
+  const size_t smem = (size_t)stages * stage_bytes + 2048;
+  switch (x_blocks) {
+    case 1: wgrad_bf16_kernel<1><<<grid, THREADS, smem, st>>>(mDy, mX, p); break;
+    case 2: wgrad_bf16_kernel<2><<<grid, THREADS, smem, st>>>(mDy, mX, p); break;
+    case 3: wgrad_bf16_kernel<3><<<grid, THREADS, smem, st>>>(mDy, mX, p); break;
+    default: wgrad_bf16_kernel<4><<<grid, THREADS, smem, st>>>(mDy, mX, p); break;
+  }
   return dp_check_launch();
 }
 
@@ -697,7 +606,7 @@ extern "C" int dp_cvt_bf16(const float* src, int64_t ld, int64_t rows, int32_t C
   const int vec_ok = (((uintptr_t)src & 15) == 0 && ld % 4 == 0) ? 1 : 0;
   const long long total = rows * (ld_dst / 8);
   long long blocks = (total + 255) / 256;
-  if (blocks > 148 * 32) blocks = 148 * 32;
+  if (blocks > g_num_sms * 32) blocks = g_num_sms * 32;
   cvt_bf16_kernel<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(src, ld, rows, C, (__nv_bfloat16*)dst, ld_dst, vec_ok);
   return dp_check_launch();
 }
@@ -708,7 +617,7 @@ extern "C" int dp_pack_conv_weight_bf16(const float* w, int32_t K, int32_t C, in
   const int Cp = wrow_bf16(C), Kp = wrow_bf16(K);
   long long total = (long long)R * S * ((long long)K * Cp > (long long)C * Kp ? (long long)K * Cp : (long long)C * Kp);
   int blocks = (int)((total + 255) / 256);
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > g_num_sms * 16) blocks = g_num_sms * 16;
   pack_bf16_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(w, K, C, R * S, Cp, Kp, (__nv_bfloat16*)kc, (__nv_bfloat16*)ck);
   return dp_check_launch();
 }

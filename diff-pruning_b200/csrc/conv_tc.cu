@@ -1,36 +1,34 @@
-// conv_tc.cu — tcgen05 / TMEM / TMA implicit-GEMM convolution for sm_100a, fp32-grade through a THREE-PRODUCT SPLIT.
+// conv_tc.cu — wgmma / TMA implicit-GEMM convolution for sm_90a, fp32-grade through a THREE-PRODUCT SPLIT.
 //
 // fprop / dgrad / attention GEMMs (conv_tc_ps_kernel): 3 x FP16.  Every operand is scaled by a power of two taken from its "amax slot"
 // (an upper bound of max|v|: dp_amax for activations / gradients, dp_pack_conv_weight_tc for weights) so that |s*v| < 2^14, then
 //     s*v = hi + lo,   hi = fp16(s*v) (11 significant bits),  lo' = fp16((s*v - hi) * 2^11)            (22 bits kept, as 3xTF32 does)
 //     x*w ~= [hi(x)*hi(w)] + 2^-11 * [hi(x)*lo'(w) + lo'(x)*hi(w)]
-// with both brackets accumulated in fp32 in TMEM (main | correction accumulator) by tcgen05.mma kind::f16 — twice the rate of
-// kind::tf32 and half the shared-memory operand bytes, which is what bounded the 3xTF32 kernel (profiles/r02_experiments.md).  Elements
-// more than 2^28 below the tensor's maximum lose RELATIVE precision (absolute error <= 2^-50 of the maximum): below fp32 round-off of any
-// sum they take part in.
+// with both brackets accumulated in fp32 registers (main | correction accumulator) by wgmma on fp16 operands — twice the rate of
+// tf32 wgmma and half the shared-memory operand bytes.  Elements more than 2^28 below the tensor's maximum lose RELATIVE precision
+// (absolute error <= 2^-50 of the maximum): below fp32 round-off of any sum they take part in.
 // The weight gradient (wgrad_tc_kernel) uses the same split with both operands scaled by their own slots.
 //
 // GEMM view: M = N*H*W output pixels (tile of 128 = one TMA box of the NHWC activation), N = output channels, K = taps x input
 // channels, one pipeline stage = (one tap, 64 channels).  The activation box is im2col-free: the tap shift is a coordinate offset,
 // image borders are TMA out-of-bounds zero fill, stride 2 is a TMA element stride.
 //
-// Kernels:
-//   conv_tc_ps_kernel     fprop / dgrad / NT GEMM: persistent (1 CTA per SM loops over (tile, K split) work items), the raw fp32 A boxes
-//                         are split IN PLACE into fp16 hi | lo' tiles by 4 warps, B = pre-split fp16 weights by TMA, 3 x 64 KB stages,
-//                         two TMEM accumulator sets (the epilogue of tile i overlaps the main loop of tile i+1), and
-//                         a_hi x [b_hi | b_lo'] issued as ONE N=256 instruction into [main | correction]
+// Kernels (warpgroup roles: sm90.cuh):
+//   conv_tc_ps_kernel     fprop / dgrad / NT GEMM: persistent (1 CTA per SM loops over (tile, K split) work items); each consumer
+//                         warpgroup splits its 64 rows of the raw fp32 A boxes IN PLACE into fp16 hi | lo' tiles, B = pre-split fp16
+//                         weights by TMA, 3 x 64 KB stages
 //   splitk_epilogue_kernel  fixed-order sum of the K splits + the epilogue (small-M launches)
-//   wgrad_tc_kernel       weight gradient: dY^T split into TMEM (TS mode), X split in place in shared memory, both MN-major, 64-pixel
-//                         stages, split-K over pixels
+//   wgrad_tc_kernel       weight gradient: dY and X both split in place in shared memory, both MN-major, 64-pixel stages, split-K
+//                         over pixels
 //   pack / split / transpose helpers; dp_gemm_nt_tc runs the attention GEMMs on the persistent kernel.
-// History (git tags): `lab-kernels-r01` round-1 experimental variants; `lab-pair-kernel-r02` the cta_group::2 CTA-pair kernel (correct,
-// 1.4x slower); `tf32x3-r02` the all-3xTF32 build this file replaced.
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <mutex>
 #include "common.cuh"
+#include "sm90.cuh"
 
 namespace {
+using namespace sm90;
 
 constexpr int BM = 128, BK = 64;          // pixel tile, K elements (channels of one tap) per pipeline stage
 constexpr int A_BYTES = BM * 32 * 4;      // 16 KB: one raw fp32 TMA box of 32 channels = one fp16 tile of 64 channels
@@ -57,8 +55,8 @@ struct TcParams {
   const uint32_t* amax_b;
   uint32_t* amax_out;       // optional amax slot of the output tensor
   // split-K (persistent kernel, launches with fewer tiles than half the SMs: the 4x4 / 8x8 / 16x16 levels): work item = (tile, K split);
-  // a split walks `it_per_split` pipeline stages of the tile and writes its raw accumulator to ws[split][row][channel]
-  // (row = tile_m * 128 + TMEM lane, pitch ws_ld); splitk_epilogue_kernel sums the splits in fixed order and applies the epilogue
+  // a split walks `it_per_split` pipeline stages of the tile and writes its accumulator to ws[split][row][channel]
+  // (row = tile_m * 128 + tile row, pitch ws_ld); splitk_epilogue_kernel sums the splits in fixed order and applies the epilogue
   int ksplit, it_per_split;
   float* ws; long long ws_split_stride; int ws_ld;
 };
@@ -97,26 +95,6 @@ __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* map
       ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
 }
-// K-major, 128B-swizzled operand tile descriptor (cute::UMMA::SmemDescriptor): start>>4 | LBO(1)<<16 | SBO(1024B>>4)<<32
-// | version(1)<<46 | layout SWIZZLE_128B(2)<<61
-__device__ __forceinline__ uint64_t umma_desc(uint32_t saddr) {
-  return (uint64_t)((saddr & 0x3FFFF) >> 4) | (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
-}
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t acc) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(acc)
-      : "memory");
-}
-// A operand from TENSOR memory (packed fp16 pairs, 8 columns per 16-element K step)
-__device__ __forceinline__ void umma_f16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc, uint32_t idesc, uint32_t acc) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"(acc)
-      : "memory");
-}
 // amax slot -> power-of-two scale.  E = biased exponent of the bound (|v| < 2^(E-126)), clamped so that both factors are normal floats;
 // up = 2^(140-E) brings the operand below 2^14 (fp16 overflows at 65504), dn = 2^(E-140) undoes it in the epilogue.
 __device__ __forceinline__ int amax_exponent(const uint32_t* slot) {
@@ -134,101 +112,38 @@ __device__ __forceinline__ void split2(float a, float b, uint32_t& h, uint32_t& 
   h = *reinterpret_cast<const uint32_t*>(&hh);
   l = *reinterpret_cast<const uint32_t*>(&ll);
 }
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-// warp-converged single-lane election (elect.sync): lets ptxas keep descriptors / barrier addresses in UNIFORM registers and emit
-// straight-line UTCHMMA / UTMALDG; a plain `if (lane == 0)` makes it wrap every such instruction in an ELECT / BRA.U.ANY loop.
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile("{\n\t.reg .pred P1;\n\telect.sync _|P1, 0xffffffff;\n\tselp.u32 %0, 1, 0, P1;\n\t}" : "=r"(pred));
-  return pred != 0;
-}
-// A whole (converged) warp waits on a barrier (every lane polls: hardware-suspended try_wait; lane-0-only polling measured 14 % slower).
-__device__ __forceinline__ void mbar_wait_warp(uint32_t bar, uint32_t parity) { mbar_wait(bar, parity); }
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-      ::"r"(taddr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]),
-        "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]), "r"(v[16]), "r"(v[17]), "r"(v[18]), "r"(v[19]),
-        "r"(v[20]), "r"(v[21]), "r"(v[22]), "r"(v[23]), "r"(v[24]), "r"(v[25]), "r"(v[26]), "r"(v[27]), "r"(v[28]), "r"(v[29]),
-        "r"(v[30]), "r"(v[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};"
-      ::"r"(taddr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]),
-        "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {   // caller issues tcgen05.wait::ld
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-        "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-        "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr));
+// one scaled fp32 value -> fp16 hi and lo' = (v - hi) * 2^11
+__device__ __forceinline__ void split1(float v, __half& h, __half& l) {
+  h = __float2half_rn(v);
+  l = __float2half_rn((v - __half2float(h)) * LO_SCALE);
 }
 
-// ------------------------------------------------------------------------------------------------ persistent variant
-// One CTA per SM loops over (tile, K split) work items (static stride), 10 warps: TMA producer | MMA issuer | 4 splitter warps |
-// 4 epilogue warps.  Stage in shared memory = [A box k 0..31 | A box k 32..63 | b_hi | b_lo'] x 16 KB.  Splitter thread <-> pixel row
-// reads its 64 raw floats (2 x 128 B, TMA 128B-swizzled: conflict-free for a quarter warp), scales and splits them.  Two operand paths:
-//   TS = false  the row's 64 fp16 hi / 64 lo' values overwrite the same two 128-byte rows IN PLACE (K-major SWIZZLE_128B tiles, no
-//               second buffer, no cross-thread hazard); SS-mode MMA.  TMEM = two accumulator sets (2 x [main 128 | correction 128]),
-//               so the epilogue of tile i overlaps the main loop of tile i+1.  Shared-memory traffic per stage: 64 KB TMA writes + 64 KB
-//               splitter + 80 KB MMA operand reads (measured: L1/TEX 72 % busy — the limiter, profiles/r02_experiments.md).
-//   TS = true   hi / lo' go to TENSOR memory with tcgen05.st (thread = TMEM lane) and the MMA takes A from TMEM: 64 + 32 + 48 KB per
-//               stage.  The A stages take the TMEM columns of the second accumulator set ([0,256) accumulators | 256 + 64 s: a_hi 32
-//               a_lo' 32), so the epilogue drains the single set into registers first and hands it back before touching global memory.
-// launch_tc picks TS for long K loops (>= 9 stages per work item: the 3x3 convolutions, + 7-15 % on the big layers) and the
-// double-buffered SS form for short ones (1x1 convolutions / linears: 4-stage tiles lose more to the accumulator hand-over than they gain).
-constexpr int PS_THREADS = 320, PS_STAGES = 3;
-constexpr int PS_TS_MIN_STAGES = 9;     // K-loop length (stages per work item) from which the TS operand path wins
+// ------------------------------------------------------------------------------------------------ persistent fprop / dgrad / NT GEMM
+// Stage = [A box k 0..31 | A box k 32..63 | b_hi | b_lo'] x 16 KB.  Consumer warpgroup c splits its tile rows 64c .. 64c+63 IN PLACE
+// (thread = row, raw box), then main += a_hi b_hi, corr += a_hi b_lo' + a_lo' b_hi per 16-element K step.  One wgmma group stays in
+// flight, so a warpgroup splits stage i+1 while the tensor cores run stage i.
+constexpr int PS_STAGES = 3, PS_BN = 128;
+constexpr int PS_B_BYTES = PS_BN * BK * 2;
+constexpr int PS_STAGE_BYTES = 2 * A_BYTES + 2 * PS_B_BYTES;
 
-template <bool TS>
-__global__ void __launch_bounds__(PS_THREADS, 1)
+__global__ void __launch_bounds__(THREADS, 1)
 conv_tc_ps_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapBh,
                   const __grid_constant__ CUtensorMap mapBl, const TcParams p, const int tiles_m, const int total_tiles) {
   const int total_work = total_tiles * p.ksplit;     // work item wi = split * total_tiles + tile (the splits of one tile run on different SMs)
-  constexpr int BN = 128;
-  constexpr int B_BYTES = BN * BK * 2;
-  constexpr int STAGE_BYTES = 2 * A_BYTES + 2 * B_BYTES;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t pad_to = ((raw + 1023u) & ~1023u) - raw;
   uint8_t* smem = smem_raw + pad_to;
   const uint32_t sbase = raw + pad_to;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + PS_STAGES * STAGE_BYTES);
-  const uint32_t bar0 = sbase + PS_STAGES * STAGE_BYTES;
+  const uint32_t bar0 = sbase + PS_STAGES * PS_STAGE_BYTES;
   auto full_bar = [&](int s) { return bar0 + 8u * s; };
-  auto conv_bar = [&](int s) { return bar0 + 8u * (PS_STAGES + s); };
-  auto empty_bar = [&](int s) { return bar0 + 8u * (2 * PS_STAGES + s); };
-  auto tfull_bar = [&](int b) { return bar0 + 8u * (3 * PS_STAGES + b); };
-  auto tempty_bar = [&](int b) { return bar0 + 8u * (3 * PS_STAGES + 2 + b); };
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 3 * PS_STAGES + 4);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  auto empty_bar = [&](int s) { return bar0 + 8u * (PS_STAGES + s); };
+  const int wg = threadIdx.x >> 7, tid = threadIdx.x & 127;
   if (threadIdx.x == 0) {
-    for (int s = 0; s < PS_STAGES; ++s) { mbar_init(full_bar(s), 1); mbar_init(conv_bar(s), 128); mbar_init(empty_bar(s), 1); }
-    for (int b = 0; b < 2; ++b) { mbar_init(tfull_bar(b), 1); mbar_init(tempty_bar(b), 128); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    for (int s = 0; s < PS_STAGES; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 8); }   // one arrival per consumer warp
+    mbar_init_fence();
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(512) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_slot;
   const int iters_per_tile = p.ntaps * p.kchunks;
 
   auto tile_coords = [&](int tile, int& q0, int& p0, int& n0, int& nblk) {
@@ -240,11 +155,10 @@ conv_tc_ps_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constan
     q0 = tw * p.bw; p0 = th * p.bh; n0 = tn * p.bn;
   };
 
-  if (warp == 0) {
-    if (lane == 0) {
-      asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&mapA)) : "memory");
-      asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&mapBh)) : "memory");
-      asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&mapBl)) : "memory");
+  if (wg == 0) {
+    setmaxnreg_dec<40>();
+    if (threadIdx.x == 0) {
+      prefetch_map(&mapA); prefetch_map(&mapBh); prefetch_map(&mapBl);
       uint32_t g = 0;
       for (int wi = blockIdx.x; wi < total_work; wi += gridDim.x) {
         const int tile = wi % total_tiles, it0 = (wi / total_tiles) * p.it_per_split, it1 = min(iters_per_tile, it0 + p.it_per_split);
@@ -254,308 +168,132 @@ conv_tc_ps_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constan
           const int s = g % PS_STAGES;
           const uint32_t ph = (g / PS_STAGES) & 1u;
           mbar_wait(empty_bar(s), ph ^ 1u);
-          mbar_expect_tx(full_bar(s), 2 * A_BYTES + 2 * B_BYTES);
+          mbar_expect_tx(full_bar(s), PS_STAGE_BYTES);
           const int tap = it / p.kchunks, kc = it - tap * p.kchunks;
-          const uint32_t st = sbase + s * STAGE_BYTES;
+          const uint32_t st = sbase + s * PS_STAGE_BYTES;
           const int aw = q0 * p.in_stride + p.dw[tap], ah = p0 * p.in_stride + p.dh[tap];
           tma_load_4d(st, &mapA, full_bar(s), kc * BK, aw, ah, n0);
           tma_load_4d(st + A_BYTES, &mapA, full_bar(s), kc * BK + 32, aw, ah, n0);     // past the last channel: TMA zero fill
           const int tapb = p.b_from_img ? n0 : p.wt[tap];
-          tma_load_3d(st + 2 * A_BYTES, &mapBh, full_bar(s), kc * BK, nblk * BN, tapb);
-          tma_load_3d(st + 2 * A_BYTES + B_BYTES, &mapBl, full_bar(s), kc * BK, nblk * BN, tapb);
+          tma_load_3d(st + 2 * A_BYTES, &mapBh, full_bar(s), kc * BK, nblk * PS_BN, tapb);
+          tma_load_3d(st + 2 * A_BYTES + PS_B_BYTES, &mapBl, full_bar(s), kc * BK, nblk * PS_BN, tapb);
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      uint32_t g = 0, tl = 0;
-      for (int wi = blockIdx.x; wi < total_work; wi += gridDim.x, ++tl) {
-        const int tile = wi % total_tiles, it0 = (wi / total_tiles) * p.it_per_split, it1 = min(iters_per_tile, it0 + p.it_per_split);
-        const int nblk = tile / tiles_m;
-        const int n_valid = min(BN, p.Nout - nblk * BN);
-        const uint32_t n_instr = (uint32_t)((n_valid + 15) & ~15);
-        // kind::f16 instruction descriptor: D = fp32 (bit 4), A / B format 0 = fp16, both K-major, N >> 3 at bit 17, M >> 4 at bit 24
-        const uint32_t idesc = (1u << 4) | ((n_instr >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
-        const uint32_t idesc256 = (1u << 4) | ((256u >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
-        if constexpr (TS) {
-          mbar_wait(tempty_bar(0), (tl & 1u) ^ 1u);           // epilogue has drained the accumulators of the previous tile
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-          const uint32_t acc = tmem_base;
-          for (int it = it0; it < it1; ++it, ++g) {
-            const int s = g % PS_STAGES;
-            const uint32_t ph = (g / PS_STAGES) & 1u;
-            mbar_wait(conv_bar(s), ph);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            const uint32_t st = sbase + s * STAGE_BYTES;
-  #pragma unroll
-            const uint32_t a_t = tmem_base + 256u + 64u * (uint32_t)s;
-  #pragma unroll
-            for (int k = 0; k < BK / 16; ++k) {      // one instruction = 16 fp16 along K = 8 packed TMEM columns of A, 32 bytes of every B row
-              const uint64_t b_hi = umma_desc(st + 2 * A_BYTES + k * 32);
-              const uint32_t first = (it > it0 || k > 0) ? 1u : 0u;
-              // a_hi x [b_hi | b_lo'] -> [main | correction] as ONE N=256 instruction (the two B tiles are adjacent in shared memory)
-              umma_f16_ts(acc, a_t + k * 8, b_hi, idesc256, first);
-              umma_f16_ts(acc + 128, a_t + 32 + k * 8, b_hi, idesc, 1u);
-            }
-            umma_commit(empty_bar(s));
-          }
-          umma_commit(tfull_bar(0));
+    return;
+  }
+  setmaxnreg_inc<232>();
+  const int c = wg - 1;                              // consumer warpgroup: tile rows 64c .. 64c + 63
+  const int warp = tid >> 5, lane = tid & 31;
+  const int r = 64 * c + (tid & 63), h = tid >> 6;   // splitter task: row r, raw box h (K elements 32h .. 32h + 31 of the stage)
+  const uint32_t sw = (uint32_t)(r & 7);             // 128B swizzle: 16-byte chunk j of row r sits at chunk position j ^ (r & 7)
+  const float sa = scale_up(amax_exponent(p.amax_a));
+  // accumulators hold (s_a s_b) x the products: f1 * f2 undoes the two power-of-two operand scales (two factors: their product may underflow)
+  const float f1 = scale_dn(amax_exponent(p.amax_a)), f2 = scale_dn(amax_exponent(p.amax_b)) * p.alpha;
+  auto fin = [&](float main, float corr) { return fmaf(corr, LO_UNSCALE, main) * f1 * f2; };
+  float amax = 0.f;         // max |value written| by this thread (split launches: splitk_epilogue_kernel writes, and tracks, the outputs)
+  uint32_t g = 0;
+  for (int wi = blockIdx.x; wi < total_work; wi += gridDim.x) {
+    const int tile = wi % total_tiles, it0 = (wi / total_tiles) * p.it_per_split, it1 = min(iters_per_tile, it0 + p.it_per_split);
+    float acc[64], cor[64];
+    int prev_s = 0;
+    for (int it = it0; it < it1; ++it, ++g) {
+      const int s = g % PS_STAGES;
+      const uint32_t ph = (g / PS_STAGES) & 1u;
+      mbar_wait(full_bar(s), ph);
+      uint8_t* a0 = smem + s * PS_STAGE_BYTES + r * 128;      // row r of the k 0..31 box  -> row r of a_hi
+      uint8_t* a1 = a0 + A_BYTES;                              // row r of the k 32..63 box -> row r of a_lo'
+      const uint8_t* src = h ? a1 : a0;
+      float4 v[8];
+#pragma unroll
+      for (int j = 0; j < 8; ++j) v[j] = *reinterpret_cast<const float4*>(src + ((j ^ sw) << 4));
+      named_sync(1 + c, 128);                                  // both halves of every row of this warpgroup have read it
+#pragma unroll
+      for (int m = 0; m < 4; ++m) {        // output chunk 4h + m = K elements 32h + 8m .. 32h + 8m + 7
+        const float4 x0 = v[2 * m], x1 = v[2 * m + 1];
+        uint4 hq, lq;
+        split2(x0.x * sa, x0.y * sa, hq.x, lq.x);
+        split2(x0.z * sa, x0.w * sa, hq.y, lq.y);
+        split2(x1.x * sa, x1.y * sa, hq.z, lq.z);
+        split2(x1.z * sa, x1.w * sa, hq.w, lq.w);
+        const uint32_t pos = (uint32_t)(((4 * h + m) ^ sw) << 4);
+        *reinterpret_cast<uint4*>(a0 + pos) = hq;
+        *reinterpret_cast<uint4*>(a1 + pos) = lq;
+      }
+      fence_proxy_async();
+      named_sync(1 + c, 128);                                  // the warpgroup's 64 rows are split
+      const uint32_t st = sbase + s * PS_STAGE_BYTES;
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < BK / 16; ++k) {      // one instruction = 16 fp16 along K = 32 bytes of every 128-byte row
+        const uint64_t a_hi = desc_k(st + c * 8192 + k * 32), a_lo = desc_k(st + A_BYTES + c * 8192 + k * 32);
+        const uint64_t b_hi = desc_k(st + 2 * A_BYTES + k * 32), b_lo = desc_k(st + 2 * A_BYTES + PS_B_BYTES + k * 32);
+        const uint32_t first = (it > it0 || k > 0) ? 1u : 0u;
+        wgmma_f16_n128<0, 0>(acc, a_hi, b_hi, first);
+        wgmma_f16_n128<0, 0>(cor, a_hi, b_lo, first);
+        wgmma_f16_n128<0, 0>(cor, a_lo, b_hi, 1u);
+      }
+      wgmma_commit();
+      wgmma_wait<1>();                        // the previous stage's MMAs have read their operands: hand it back to TMA
+      if (it > it0 && lane == 0) mbar_arrive(empty_bar(prev_s));
+      prev_s = s;
+    }
+    wgmma_wait<0>();
+    fence_regs(acc); fence_regs(cor);
+    if (lane == 0) mbar_arrive(empty_bar(prev_s));
+
+    int q0, p0, n0, nblk;
+    tile_coords(tile, q0, p0, n0, nblk);
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const int row = 64 * c + 16 * warp + (lane >> 2) + 8 * i;
+      const int cb = 2 * (lane & 3);
+      if (p.ksplit > 1) {   // split-K: partial sums into this split's slab of the (padded) workspace; splitk_epilogue_kernel finishes
+        float* wrow = p.ws + (long long)(wi / total_tiles) * p.ws_split_stride + ((long long)(tile - nblk * tiles_m) * BM + row) * p.ws_ld + nblk * PS_BN;
+#pragma unroll
+        for (int j = 0; j < 16; ++j)
+          *reinterpret_cast<float2*>(wrow + 8 * j + cb) =
+              make_float2(fin(acc[4 * j + 2 * i], cor[4 * j + 2 * i]), fin(acc[4 * j + 2 * i + 1], cor[4 * j + 2 * i + 1]));
+        continue;
+      }
+      const int w_l = row % p.bw, h_l = (row / p.bw) % p.bh, n_l = row / (p.bw * p.bh);
+      const int img = n0 + n_l;
+      if (img >= p.Nimg) continue;
+      const long long m = ((long long)img * p.Ho + ((p0 + h_l) * p.os + p.oa)) * p.Wo + ((q0 + w_l) * p.os + p.ob);
+      float* yrow = p.y + m * p.ldy;
+      const float* rrow = p.residual ? p.residual + m * p.ld_res : nullptr;
+      const float* arow2 = p.rowadd ? p.rowadd + (long long)img * p.ld_rowadd : nullptr;
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        const int col = nblk * PS_BN + 8 * j + cb;
+        float o[2] = {fin(acc[4 * j + 2 * i], cor[4 * j + 2 * i]), fin(acc[4 * j + 2 * i + 1], cor[4 * j + 2 * i + 1])};
+        if (p.vec4 && col + 2 <= p.Nout) {
+          if (p.bias) { const float2 t = __ldg(reinterpret_cast<const float2*>(p.bias + col)); o[0] += t.x; o[1] += t.y; }
+          if (arow2) { const float2 t = __ldg(reinterpret_cast<const float2*>(arow2 + col)); o[0] += t.x; o[1] += t.y; }
+          if (rrow) { const float2 t = __ldg(reinterpret_cast<const float2*>(rrow + col)); o[0] += t.x; o[1] += t.y; }
+          float2* dst = reinterpret_cast<float2*>(yrow + col);
+          if (p.accumulate) { const float2 t = *dst; o[0] += t.x; o[1] += t.y; }
+          *dst = make_float2(o[0], o[1]);
+          amax = fmaxf(amax, fmaxf(fabsf(o[0]), fabsf(o[1])));
         } else {
-          const uint32_t b = tl & 1u, use = tl >> 1;
-          mbar_wait(tempty_bar(b), (use & 1u) ^ 1u);          // epilogue has drained this accumulator set
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-          const uint32_t acc = tmem_base + b * 256u;
-          for (int it = it0; it < it1; ++it, ++g) {
-            const int s = g % PS_STAGES;
-            const uint32_t ph = (g / PS_STAGES) & 1u;
-            mbar_wait(conv_bar(s), ph);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            const uint32_t st = sbase + s * STAGE_BYTES;
-  #pragma unroll
-            for (int k = 0; k < BK / 16; ++k) {      // one instruction = 16 fp16 along K = 32 bytes of every 128-byte row
-              const uint64_t a_hi = umma_desc(st + k * 32), a_lo = umma_desc(st + A_BYTES + k * 32);
-              const uint64_t b_hi = umma_desc(st + 2 * A_BYTES + k * 32);
-              const uint32_t first = (it > it0 || k > 0) ? 1u : 0u;
-              // a_hi x [b_hi | b_lo'] -> [main | correction] as ONE N=256 instruction (the two B tiles are adjacent in shared memory):
-              // 8 instead of 12 instructions per stage and 5/6 of the operand reads
-              umma_f16(acc, a_hi, b_hi, idesc256, first);
-              umma_f16(acc + 128, a_lo, b_hi, idesc, 1u);
-            }
-            umma_commit(empty_bar(s));
-          }
-          umma_commit(tfull_bar(b));
-        }
-      }
-    }
-  } else if (warp < 6) {
-    if constexpr (TS) {
-      // ---- splitter warps 2..5 (TMEM lane quarter = warp & 3)
-      const int r = (warp & 3) * 32 + lane;            // pixel row of the tile = TMEM lane
-      const uint32_t lane_addr = (uint32_t)((warp & 3) * 32) << 16;
-      const uint32_t sw = (uint32_t)(r & 7);           // 128B swizzle: 16-byte chunk c of row r sits at chunk position c ^ (r & 7)
-      const float sa = scale_up(amax_exponent(p.amax_a));
-      uint32_t g = 0;
-      for (int wi = blockIdx.x; wi < total_work; wi += gridDim.x) {
-        const int it0 = (wi / total_tiles) * p.it_per_split, it1 = min(iters_per_tile, it0 + p.it_per_split);
-        for (int it = it0; it < it1; ++it, ++g) {
-          const int s = g % PS_STAGES;
-          const uint32_t ph = (g / PS_STAGES) & 1u;
-          mbar_wait(full_bar(s), ph);
-          const uint8_t* a0 = smem + s * STAGE_BYTES + r * 128;      // row r of the k 0..31 box
-          const uint8_t* a1 = a0 + A_BYTES;                          // row r of the k 32..63 box
-          uint32_t hi[32], lo[32];                                   // column j = K elements (2j, 2j+1)
-  #pragma unroll
-          for (int c = 0; c < 8; ++c) {       // a quarter warp (8 consecutive rows) touches 8 distinct chunk positions: conflict-free
-            const float4 x0 = *reinterpret_cast<const float4*>(a0 + ((c ^ sw) << 4));
-            const float4 x1 = *reinterpret_cast<const float4*>(a1 + ((c ^ sw) << 4));
-            split2(x0.x * sa, x0.y * sa, hi[2 * c], lo[2 * c]);
-            split2(x0.z * sa, x0.w * sa, hi[2 * c + 1], lo[2 * c + 1]);
-            split2(x1.x * sa, x1.y * sa, hi[16 + 2 * c], lo[16 + 2 * c]);
-            split2(x1.z * sa, x1.w * sa, hi[16 + 2 * c + 1], lo[16 + 2 * c + 1]);
-          }
-          const uint32_t a_t = tmem_base + lane_addr + 256u + 64u * (uint32_t)s;
-          tmem_st32(a_t, hi);
-          tmem_st32(a_t + 32, lo);
-          asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-          asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-          mbar_arrive(conv_bar(s));
-        }
-      }
-    } else {
-      // ---- splitter warps 2..5
-      const int r = threadIdx.x - 64;                  // pixel row of the tile
-      const uint32_t sw = (uint32_t)(r & 7);           // 128B swizzle: 16-byte chunk c of row r sits at chunk position c ^ (r & 7)
-      const float sa = scale_up(amax_exponent(p.amax_a));
-      uint32_t g = 0;
-      for (int wi = blockIdx.x; wi < total_work; wi += gridDim.x) {
-        const int it0 = (wi / total_tiles) * p.it_per_split, it1 = min(iters_per_tile, it0 + p.it_per_split);
-        for (int it = it0; it < it1; ++it, ++g) {
-          const int s = g % PS_STAGES;
-          const uint32_t ph = (g / PS_STAGES) & 1u;
-          mbar_wait(full_bar(s), ph);
-          uint8_t* a0 = smem + s * STAGE_BYTES + r * 128;      // row r of the k 0..31 box  -> row r of a_hi
-          uint8_t* a1 = a0 + A_BYTES;                          // row r of the k 32..63 box -> row r of a_lo'
-          float4 v[16];
-  #pragma unroll
-          for (int c = 0; c < 8; ++c) {       // a quarter warp (8 consecutive rows) touches 8 distinct chunk positions: conflict-free
-            v[c] = *reinterpret_cast<const float4*>(a0 + ((c ^ sw) << 4));
-            v[8 + c] = *reinterpret_cast<const float4*>(a1 + ((c ^ sw) << 4));
-          }
-  #pragma unroll
-          for (int c = 0; c < 8; ++c) {       // output chunk c = k 8c .. 8c+7
-            const float4 x0 = v[2 * c], x1 = v[2 * c + 1];
-            uint4 h, l;
-            split2(x0.x * sa, x0.y * sa, h.x, l.x);
-            split2(x0.z * sa, x0.w * sa, h.y, l.y);
-            split2(x1.x * sa, x1.y * sa, h.z, l.z);
-            split2(x1.z * sa, x1.w * sa, h.w, l.w);
-            *reinterpret_cast<uint4*>(a0 + ((c ^ sw) << 4)) = h;
-            *reinterpret_cast<uint4*>(a1 + ((c ^ sw) << 4)) = l;
-          }
-          asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-          mbar_arrive(conv_bar(s));
-        }
-      }
-    }
-  } else {
-    // ---- epilogue warps 6..9 (TMEM lane quarter = warp & 3)
-    const int q = warp & 3;
-    const int row = q * 32 + lane;
-    const uint32_t lane_addr = (uint32_t)(q * 32) << 16;
-    const int w_l = row % p.bw, h_l = (row / p.bw) % p.bh, n_l = row / (p.bw * p.bh);
-    // accumulators hold (s_a s_b) x the products: f1 * f2 undoes the two power-of-two operand scales (two factors: their product may underflow)
-    const float f1 = scale_dn(amax_exponent(p.amax_a)), f2 = scale_dn(amax_exponent(p.amax_b)) * p.alpha;
-    auto fin = [&](uint32_t main, uint32_t corr) { return fmaf(__uint_as_float(corr), LO_UNSCALE, __uint_as_float(main)) * f1 * f2; };
-    float amax = 0.f;         // max |value written| by this thread (split launches: splitk_epilogue_kernel writes, and tracks, the outputs)
-    uint32_t tl = 0;
-    for (int wi = blockIdx.x; wi < total_work; wi += gridDim.x, ++tl) {
-      const int tile = wi % total_tiles;
-      int q0, p0, n0, nblk;
-      tile_coords(tile, q0, p0, n0, nblk);
-      if constexpr (TS) {
-        mbar_wait(tfull_bar(0), tl & 1u);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const int img = n0 + n_l;
-        const bool row_ok = img < p.Nimg;
-        const long long m = ((long long)img * p.Ho + ((p0 + h_l) * p.os + p.oa)) * p.Wo + ((q0 + w_l) * p.os + p.ob);
-        float* yrow = p.y + m * p.ldy;
-        const float* rrow = p.residual ? p.residual + m * p.ld_res : nullptr;
-        const float* arow2 = p.rowadd ? p.rowadd + (long long)img * p.ld_rowadd : nullptr;
-        float out[BN];          // this thread's row of the tile: drained before anything else so the MMA warp can start the next tile
-  #pragma unroll
-        for (int j = 0; j < BN / 32; ++j) {
-          uint32_t v[32], u[32];
-          const uint32_t taddr = tmem_base + lane_addr + (uint32_t)(j * 32);
-          tmem_ld32(taddr, v);
-          tmem_ld32(taddr + 128u, u);
-          asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-  #pragma unroll
-          for (int i = 0; i < 32; ++i) out[j * 32 + i] = fin(v[i], u[i]);
-        }
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-        mbar_arrive(tempty_bar(0));
-  #pragma unroll
-        for (int j = 0; j < BN / 32; ++j) {
-          const float* oj = out + j * 32;
-          if (p.ksplit > 1) {   // split-K: partial sums into this split's slab of the (padded) workspace; splitk_epilogue_kernel finishes
-            float* wrow = p.ws + (long long)(wi / total_tiles) * p.ws_split_stride + ((long long)(tile - nblk * tiles_m) * BM + row) * p.ws_ld + nblk * BN + j * 32;
-  #pragma unroll
-            for (int i = 0; i < 32; i += 4)
-              *reinterpret_cast<float4*>(wrow + i) = make_float4(oj[i], oj[i + 1], oj[i + 2], oj[i + 3]);
-          } else if (row_ok) {
-            const int c0 = nblk * BN + j * 32;
-            if (p.vec4 && c0 + 32 <= p.Nout) {
-  #pragma unroll
-              for (int i = 0; i < 32; i += 4) {
-                float4 o = make_float4(oj[i], oj[i + 1], oj[i + 2], oj[i + 3]);
-                if (p.bias) { float4 t = __ldg(reinterpret_cast<const float4*>(p.bias + c0 + i)); o.x += t.x; o.y += t.y; o.z += t.z; o.w += t.w; }
-                if (arow2) { float4 t = __ldg(reinterpret_cast<const float4*>(arow2 + c0 + i)); o.x += t.x; o.y += t.y; o.z += t.z; o.w += t.w; }
-                if (rrow) { float4 t = __ldg(reinterpret_cast<const float4*>(rrow + c0 + i)); o.x += t.x; o.y += t.y; o.z += t.z; o.w += t.w; }
-                float4* dst = reinterpret_cast<float4*>(yrow + c0 + i);
-                if (p.accumulate) { float4 t = *dst; o.x += t.x; o.y += t.y; o.z += t.z; o.w += t.w; }
-                *dst = o;
-                amax = fmaxf(fmaxf(amax, fmaxf(fabsf(o.x), fabsf(o.y))), fmaxf(fabsf(o.z), fabsf(o.w)));
-              }
-            } else {
-  #pragma unroll
-              for (int i = 0; i < 32; ++i) {
-                const int c = c0 + i;
-                if (c < p.Nout) {
-                  float o = oj[i];
-                  if (p.bias) o += __ldg(p.bias + c);
-                  if (arow2) o += __ldg(arow2 + c);
-                  if (rrow) o += __ldg(rrow + c);
-                  if (p.accumulate) o += yrow[c];
-                  yrow[c] = o;
-                  amax = fmaxf(amax, fabsf(o));
-                }
-              }
-            }
-          }
-        }
-      } else {
-        const uint32_t b = tl & 1u, use = tl >> 1;
-        mbar_wait(tfull_bar(b), use & 1u);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const int img = n0 + n_l;
-        const bool row_ok = img < p.Nimg;
-        const long long m = ((long long)img * p.Ho + ((p0 + h_l) * p.os + p.oa)) * p.Wo + ((q0 + w_l) * p.os + p.ob);
-        float* yrow = p.y + m * p.ldy;
-        const float* rrow = p.residual ? p.residual + m * p.ld_res : nullptr;
-        const float* arow2 = p.rowadd ? p.rowadd + (long long)img * p.ld_rowadd : nullptr;
-  #pragma unroll 1
-        for (int j = 0; j < BN / 32; ++j) {
-          uint32_t v[32], u[32];
-          const uint32_t taddr = tmem_base + lane_addr + b * 256u + (uint32_t)(j * 32);
-          asm volatile(
-              "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-              "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-              "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-              : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-                "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-                "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-                "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-              : "r"(taddr));
-          asm volatile(
-              "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-              "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-              "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-              : "=r"(u[0]), "=r"(u[1]), "=r"(u[2]), "=r"(u[3]), "=r"(u[4]), "=r"(u[5]), "=r"(u[6]), "=r"(u[7]), "=r"(u[8]),
-                "=r"(u[9]), "=r"(u[10]), "=r"(u[11]), "=r"(u[12]), "=r"(u[13]), "=r"(u[14]), "=r"(u[15]), "=r"(u[16]),
-                "=r"(u[17]), "=r"(u[18]), "=r"(u[19]), "=r"(u[20]), "=r"(u[21]), "=r"(u[22]), "=r"(u[23]), "=r"(u[24]),
-                "=r"(u[25]), "=r"(u[26]), "=r"(u[27]), "=r"(u[28]), "=r"(u[29]), "=r"(u[30]), "=r"(u[31])
-              : "r"(taddr + 128u));
-          asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-          if (j == BN / 32 - 1) {   // accumulators are in registers: hand the TMEM set back to the MMA warp
-            asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-            mbar_arrive(tempty_bar(b));
-          }
-          if (p.ksplit > 1) {   // split-K: raw partial sums into this split's slab of the (padded) workspace; splitk_epilogue_kernel finishes
-            float* wrow = p.ws + (long long)(wi / total_tiles) * p.ws_split_stride + ((long long)(tile - nblk * tiles_m) * BM + row) * p.ws_ld + nblk * BN + j * 32;
-  #pragma unroll
-            for (int i = 0; i < 32; i += 4)
-              *reinterpret_cast<float4*>(wrow + i) = make_float4(fin(v[i], u[i]), fin(v[i + 1], u[i + 1]), fin(v[i + 2], u[i + 2]), fin(v[i + 3], u[i + 3]));
-          } else if (row_ok) {
-            const int c0 = nblk * BN + j * 32;
-            if (p.vec4 && c0 + 32 <= p.Nout) {
-  #pragma unroll
-              for (int i = 0; i < 32; i += 4) {
-                float4 o = make_float4(fin(v[i], u[i]), fin(v[i + 1], u[i + 1]), fin(v[i + 2], u[i + 2]), fin(v[i + 3], u[i + 3]));
-                if (p.bias) { float4 t = __ldg(reinterpret_cast<const float4*>(p.bias + c0 + i)); o.x += t.x; o.y += t.y; o.z += t.z; o.w += t.w; }
-                if (arow2) { float4 t = __ldg(reinterpret_cast<const float4*>(arow2 + c0 + i)); o.x += t.x; o.y += t.y; o.z += t.z; o.w += t.w; }
-                if (rrow) { float4 t = __ldg(reinterpret_cast<const float4*>(rrow + c0 + i)); o.x += t.x; o.y += t.y; o.z += t.z; o.w += t.w; }
-                float4* dst = reinterpret_cast<float4*>(yrow + c0 + i);
-                if (p.accumulate) { float4 t = *dst; o.x += t.x; o.y += t.y; o.z += t.z; o.w += t.w; }
-                *dst = o;
-                amax = fmaxf(fmaxf(amax, fmaxf(fabsf(o.x), fabsf(o.y))), fmaxf(fabsf(o.z), fabsf(o.w)));
-              }
-            } else {
-  #pragma unroll
-              for (int i = 0; i < 32; ++i) {
-                const int c = c0 + i;
-                if (c < p.Nout) {
-                  float o = fin(v[i], u[i]);
-                  if (p.bias) o += __ldg(p.bias + c);
-                  if (arow2) o += __ldg(arow2 + c);
-                  if (rrow) o += __ldg(rrow + c);
-                  if (p.accumulate) o += yrow[c];
-                  yrow[c] = o;
-                  amax = fmaxf(amax, fabsf(o));
-                }
-              }
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int cc = col + e;
+            if (cc < p.Nout) {
+              float ov = o[e];
+              if (p.bias) ov += __ldg(p.bias + cc);
+              if (arow2) ov += __ldg(arow2 + cc);
+              if (rrow) ov += __ldg(rrow + cc);
+              if (p.accumulate) ov += yrow[cc];
+              yrow[cc] = ov;
+              amax = fmaxf(amax, fabsf(ov));
             }
           }
         }
       }
     }
-    if (p.amax_out && p.ksplit == 1) amax_commit(p.amax_out, amax);
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   }
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512) : "memory");
-  }
+  if (p.amax_out && p.ksplit == 1) amax_commit(p.amax_out, amax);
 }
 
 // Sums the K splits of conv_tc_ps_kernel in fixed order (deterministic) and applies its epilogue: bias, per-image row, residual,
@@ -600,15 +338,11 @@ __global__ void __launch_bounds__(256) splitk_epilogue_kernel(const TcParams p, 
 
 // ------------------------------------------------------------------------------------------------ wgrad
 // dW[k][tap][c] = sum_pixels dy[pix][k] * x[pix @ tap][c]: M = out-channels (128 per tile), N = in-channels of one tap (128 per tile),
-// GEMM-K = pixels, 64 per pipeline stage.  Both operands are pixel-major fp32 activations, i.e. MN-major for this product:
-//   dy: 4 raw TMA boxes [64 px][32 ch] (128-byte rows, SWIZZLE_128B).  Thread <-> out-channel reads its channel down the 64 pixel rows
-//       (a warp reads one conflict-free 128 B row per instruction), scales, splits into fp16 hi / lo' and writes 2 x 32 packed columns
-//       of TENSOR MEMORY with tcgen05.st: the MMA then runs in TS mode (A from TMEM), so dy never goes back to shared memory.
-//   x:  4 raw boxes; the boxes of channels [64j, 64j+32) and [64j+32, 64j+64) land where the fp16 blocks x_hi[j] and x_lo'[j] will live
-//       ([hi0 | hi1 | lo0 | lo1], 8 KB each = [64 px][64 ch] fp16, MN-major SWIZZLE_128B: LBO = 8 KB between 64-channel blocks, SBO = 1 KB
-//       between 8-pixel K groups); splitter thread <-> (block j, pixel row) rewrites its two 128-byte rows in place.
-//   a_hi x [x_hi | x_lo'] -> [main | correction] is ONE N=256 instruction, a_lo' x x_hi adds to the correction half.
-// TMEM: [0,128) main acc | [128,256) correction acc | 256 + 64*s: a_hi (32 columns = 64 pixels) a_lo' (32) of stage s.
+// GEMM-K = pixels, 64 per pipeline stage.  Both operands are pixel-major fp32 activations, i.e. MN-major for this product.
+// A stage holds 8 raw TMA boxes [64 px][32 ch]: dy in [0, 32 KB), x in [32 KB, 64 KB); the boxes of channels [64j, 64j+32) and
+// [64j+32, 64j+64) land where the fp16 blocks hi[j] and lo'[j] will live ([hi0 | hi1 | lo0 | lo1], MN-major SWIZZLE_128B: LBO = 8 KB
+// between 64-channel blocks).  Consumer warpgroup c splits block c of both in place (dy: thread = channel, which also sums the bias
+// gradient; x: thread = pixel row), then main += dy_hi[c] x_hi, corr += dy_hi[c] x_lo' + dy_lo'[c] x_hi.
 // grid = (k tiles * c tiles * taps, splits): split z covers pixel chunks [z*cps, (z+1)*cps) and writes its partial
 // tile to workspace[z][k][tap*C + c]; dp_conv2d_wgrad_reduce sums splits in fixed order (deterministic).
 struct WgParams {
@@ -626,48 +360,23 @@ constexpr int WG_KPIX = 64;                  // pixels per stage
 constexpr int WG_BLK = WG_KPIX * 128;        // 8 KB: one raw fp32 box [64 px][32 ch] = one fp16 block [64 px][64 ch]
 constexpr int WG_STAGES = 3, WG_STAGE_BYTES = 8 * WG_BLK;
 
-// MN-major fp16 operand, 128B-swizzled (canonical ((8,n),(8,k)):((1,LBO),(8,SBO)) in 16-byte units): LBO = 8 KB between 64-channel
-// blocks, SBO = 1 KB between 8-pixel K groups
-__device__ __forceinline__ uint64_t umma_desc_mn(uint32_t saddr) {
-  return (uint64_t)((saddr & 0x3FFFF) >> 4) | ((uint64_t)(WG_BLK >> 4) << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
-}
-
-// warps: 0 TMA | 1, 6 MMA issuers (alternate stages) | 2-5 and 7-10: two half-groups of splitters that work on the SAME stage (pixels
-// 0..31 / 32..63 of dy, first / second raw box of every x row) + epilogue.  The ring is latency bound — period ~ (TMA latency + split +
-// MMA) / stages, r02_experiments.md section 13 — so halving the ~850-instruction split of a stage shortens every stage's chain; groups on
-// ALTERNATE stages did not (same chain) and, visiting each barrier only every second phase of a 3-stage ring, could be lapped.
-constexpr int WG_THREADS = 352;
-__global__ void __launch_bounds__(WG_THREADS, 1)
+__global__ void __launch_bounds__(THREADS, 1)
 wgrad_tc_kernel(const __grid_constant__ CUtensorMap mapDy, const __grid_constant__ CUtensorMap mapX, const WgParams p) {
-  constexpr int WSTAGES = WG_STAGES;
-  constexpr int STAGE_BYTES = WG_STAGE_BYTES;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t pad_to = ((raw + 1023u) & ~1023u) - raw;
   uint8_t* smem = smem_raw + pad_to;
   const uint32_t sbase = raw + pad_to;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + WSTAGES * STAGE_BYTES);
-  const uint32_t bar0 = sbase + WSTAGES * STAGE_BYTES;
+  const uint32_t bar0 = sbase + WG_STAGES * WG_STAGE_BYTES;
   auto full_bar = [&](int s) { return bar0 + 8u * s; };
-  auto conv_bar = [&](int s) { return bar0 + 8u * (WSTAGES + s); };
-  auto empty_bar = [&](int s) { return bar0 + 8u * (2 * WSTAGES + s); };
-  const uint32_t tmem_full_bar = bar0 + 8u * (3 * WSTAGES);
-  auto iss_bar = [&](int s) { return bar0 + 8u * (3 * WSTAGES + 1 + s); };
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 4 * WSTAGES + 1);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  auto empty_bar = [&](int s) { return bar0 + 8u * (WG_STAGES + s); };
+  float* bsh = reinterpret_cast<float*>(smem + WG_STAGES * WG_STAGE_BYTES + 8 * 2 * WG_STAGES);   // 128 floats: the bias sums' halves meet here
+  const int wg = threadIdx.x >> 7, tid = threadIdx.x & 127;
   if (threadIdx.x == 0) {
-    for (int s = 0; s < WSTAGES; ++s) { mbar_init(full_bar(s), 1); mbar_init(conv_bar(s), 256); mbar_init(empty_bar(s), 1); mbar_init(iss_bar(s), 1); }
-    mbar_init(tmem_full_bar, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    for (int s = 0; s < WG_STAGES; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 8); }
+    mbar_init_fence();
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(512) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_slot;
 
   const int T = p.R * p.S;
   int tile = blockIdx.x;
@@ -682,13 +391,13 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap mapDy, const __grid_constant
   // split — their accumulator rows / columns are never stored, so whatever the stage buffers still hold there is harmless
   const int dy_boxes = min(4, (p.K - kt * 128 + 31) >> 5), x_boxes = min(4, (p.C - ct * 128 + 31) >> 5);
 
-  if (warp == 0) {
-    if (lane == 0) {
-      asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&mapDy)) : "memory");
-      asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&mapX)) : "memory");
+  if (wg == 0) {
+    setmaxnreg_dec<40>();
+    if (threadIdx.x == 0) {
+      prefetch_map(&mapDy); prefetch_map(&mapX);
       for (int it = 0; it < num_iters; ++it) {
-        const int s = it % WSTAGES;
-        const uint32_t ph = (uint32_t)(it / WSTAGES) & 1u;
+        const int s = it % WG_STAGES;
+        const uint32_t ph = (uint32_t)(it / WG_STAGES) & 1u;
         mbar_wait(empty_bar(s), ph ^ 1u);
         mbar_expect_tx(full_bar(s), (uint32_t)((dy_boxes + x_boxes) * WG_BLK));
         const int chunk = chunk0 + it;
@@ -696,154 +405,128 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap mapDy, const __grid_constant
         const int th = (chunk / p.tiles_w) % p.tiles_h;
         const int tn = chunk / (p.tiles_w * p.tiles_h);
         const int q0 = tw * p.bw, p0 = th * p.bh, n0 = tn * p.bn;
-        const uint32_t st = sbase + s * STAGE_BYTES;
+        const uint32_t st = sbase + s * WG_STAGE_BYTES;
         const int xw = q0 * p.in_stride + sx - p.pad, xh = p0 * p.in_stride + r - p.pad;
 #pragma unroll
-        for (int b = 0; b < 4; ++b)     // dy: up to 4 boxes of 32 out-channels
-          if (b < dy_boxes) tma_load_4d(st + b * WG_BLK, &mapDy, full_bar(s), kt * 128 + b * 32, q0, p0, n0);
-#pragma unroll
-        for (int j = 0; j < 2; ++j) {   // x: channels [64j, 64j+32) -> future x_hi[j], [64j+32, 64j+64) -> future x_lo'[j]
-          if (2 * j < x_boxes) tma_load_4d(st + (4 + j) * WG_BLK, &mapX, full_bar(s), ct * 128 + 64 * j, xw, xh, n0);
-          if (2 * j + 1 < x_boxes) tma_load_4d(st + (6 + j) * WG_BLK, &mapX, full_bar(s), ct * 128 + 64 * j + 32, xw, xh, n0);
+        for (int b = 0; b < 4; ++b) {   // box b = channels [32b, 32b+32) of the tile -> block b >> 1, raw half b & 1
+          const uint32_t slot = (uint32_t)((b & 1) * 2 + (b >> 1));
+          if (b < dy_boxes) tma_load_4d(st + slot * WG_BLK, &mapDy, full_bar(s), kt * 128 + b * 32, q0, p0, n0);
+          if (b < x_boxes) tma_load_4d(st + (4 + slot) * WG_BLK, &mapX, full_bar(s), ct * 128 + b * 32, xw, xh, n0);
         }
       }
     }
-  } else if (warp == 1 || warp == 6) {
-    // two issuer warps on alternate stages (a lone issuer cannot run ahead of the tensor queue, profiles/r01_experiments.md),
-    // warp-converged with one elected lane
-    const uint32_t mw = (warp == 1) ? 0u : 1u;
-    // kind::f16, D = fp32, A = fp16 from TMEM, B = fp16 MN-major (bit 16)
-    const uint32_t idesc = (1u << 4) | (1u << 16) | ((uint32_t)(128 >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-    const uint32_t idesc256 = (1u << 4) | (1u << 16) | ((uint32_t)(256 >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-    if (num_iters == 0 && mw == 0) {   // empty split: release the epilogue (it writes zeros)
-      if (elect_one()) umma_commit(tmem_full_bar);
-      __syncwarp();
-    }
-    for (int it = 0; it < num_iters; ++it) {
-      if (((uint32_t)it & 1u) != mw) continue;
-      const int s = it % WSTAGES;
-      const uint32_t ph = (uint32_t)(it / WSTAGES) & 1u;
-      mbar_wait_warp(conv_bar(s), ph);
-      mbar_wait_warp(full_bar(s), ph);
-      if (it > 0) mbar_wait_warp(iss_bar((it - 1) % WSTAGES), (uint32_t)((it - 1) / WSTAGES) & 1u);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const uint32_t st = sbase + s * STAGE_BYTES;
-      const uint32_t a_t = tmem_base + 256u + 64u * s;
-      if (elect_one()) {
-#pragma unroll
-        for (int k = 0; k < WG_KPIX / 16; ++k) {     // 16 pixels per instruction = 8 packed TMEM columns of A, two 8-pixel groups (2 KB) of B
-          const uint64_t b_hi = umma_desc_mn(st + 4 * WG_BLK + k * 2048);
-          const uint32_t first = (it > 0 || k > 0) ? 1u : 0u;
-          umma_f16_ts(tmem_base, a_t + k * 8, b_hi, idesc256, first);
-          umma_f16_ts(tmem_base + 128, a_t + 32 + k * 8, b_hi, idesc, 1u);
-        }
-        umma_commit(empty_bar(s));
-        if (it == num_iters - 1) umma_commit(tmem_full_bar);
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-        mbar_arrive(iss_bar(s));
-      }
-      __syncwarp();
-    }
-  } else {
-    const int half = warp > 6 ? 1 : 0;        // splitter half-group
-    const int tid = threadIdx.x - (half ? 224 : 64);
-    const int q = warp & 3;                   // TMEM lane quarter == 32-channel box of dy (each half-group covers the four quarters)
-    const uint32_t lane_addr = (uint32_t)(q * 32) << 16;
-    const int Ey = amax_exponent(p.amax_y), Ex = amax_exponent(p.amax_x);
-    const float sy = scale_up(Ey), sxs = scale_up(Ex);
-    const int xj = tid >> 6, xp = tid & 63;   // x task of this thread: 64-channel block, pixel row; `half` picks the raw box of the row
-    const uint32_t xsw = (uint32_t)(xp & 7);
-    float bsum = 0.f;                         // sum of this thread's out-channel of dy over its pixels of the split (bias gradient)
-    float* bsh = reinterpret_cast<float*>(tmem_slot + 2);      // 128 floats behind the barriers: the halves' bias sums meet here
-    for (int it = 0; it < num_iters; ++it) {
-      const int s = it % WSTAGES;
-      const uint32_t ph = (uint32_t)(it / WSTAGES) & 1u;
-      mbar_wait(full_bar(s), ph);
-      // (1) dy^T -> TMEM: channel `lane` of box q, pixel rows 32 half .. 32 half + 31; 16-byte chunk j of row `pix` sits at position j ^ (pix & 7)
-      if (q < dy_boxes) {
-        const uint8_t* blk = smem + s * STAGE_BYTES + q * WG_BLK + half * 32 * 128 + (lane & 3) * 4;
-        uint32_t hi[16], lo[16];
-        float ssum = 0.f;
-#pragma unroll
-        for (int j = 0; j < 16; ++j) {
-          const float v0 = *reinterpret_cast<const float*>(blk + (2 * j) * 128 + ((((lane >> 2) ^ (2 * j)) & 7) << 4));
-          const float v1 = *reinterpret_cast<const float*>(blk + (2 * j + 1) * 128 + ((((lane >> 2) ^ (2 * j + 1)) & 7) << 4));
-          split2(v0 * sy, v1 * sy, hi[j], lo[j]);      // TMEM column 16 half + j = pixels (2j, 2j+1) of this half, low half first
-          ssum += v0 + v1;
-        }
-        bsum += ssum;
-        const uint32_t a_t = tmem_base + lane_addr + 256u + 64u * s + 16u * half;
-        tmem_st16(a_t, hi);
-        tmem_st16(a_t + 32, lo);
-      }
-      // (2) x: row xp of block xj.  This thread reads the row's raw box `half` (channels 32 half .. 32 half + 31 of the block); once BOTH
-      //     halves have read, it writes chunks 4 half .. 4 half + 3 of the fp16 x_hi row (over box 0) and of the x_lo' row (over box 1)
-      {
-        uint8_t* a0 = smem + s * STAGE_BYTES + (4 + xj) * WG_BLK + xp * 128;
-        uint8_t* a1 = a0 + 2 * WG_BLK;
-        const uint8_t* src = half ? a1 : a0;
-        const bool x_valid = 2 * xj + half < x_boxes;
-        float4 v[8];
-        if (x_valid) {
-#pragma unroll
-          for (int c = 0; c < 8; ++c) v[c] = *reinterpret_cast<const float4*>(src + ((c ^ xsw) << 4));
-        }
-        asm volatile("bar.sync 1, 256;" ::: "memory");
-        if (x_valid)
-#pragma unroll
-        for (int c = 0; c < 4; ++c) {
-          const float4 x0 = v[2 * c], x1 = v[2 * c + 1];
-          uint4 h, l;
-          split2(x0.x * sxs, x0.y * sxs, h.x, l.x);
-          split2(x0.z * sxs, x0.w * sxs, h.y, l.y);
-          split2(x1.x * sxs, x1.y * sxs, h.z, l.z);
-          split2(x1.z * sxs, x1.w * sxs, h.w, l.w);
-          const uint32_t pos = (uint32_t)(((4 * half + c) ^ xsw) << 4);
-          *reinterpret_cast<uint4*>(a0 + pos) = h;
-          *reinterpret_cast<uint4*>(a1 + pos) = l;
-        }
-      }
-      asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      mbar_arrive(conv_bar(s));
-    }
-    if (half) bsh[q * 32 + lane] = bsum;
-    asm volatile("bar.sync 1, 256;" ::: "memory");
-    if (!half) bsum += bsh[q * 32 + lane];
-    mbar_wait(tmem_full_bar, 0);
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const float f1 = scale_dn(Ey), f2 = scale_dn(Ex);
-    const int row = q * 32 + lane;            // k_out within the tile
-    const int kout = kt * 128 + row;
-    const long long TC_ = (long long)T * p.C;
-    float* wrow = p.ws + ((long long)blockIdx.y * p.K + kout) * TC_ + (long long)tap * p.C;
-    if (p.bias_ws && !half && tap == 0 && ct == 0 && kout < p.K) p.bias_ws[(long long)blockIdx.y * p.K + kout] = bsum;   // 0 for an empty split
-    // epilogue: half-group 0 drains accumulator columns [0, 64), half-group 1 [64, 128)
-    if (num_iters == 0) {                     // nothing was accumulated (TMEM holds garbage): this split contributes zeros
-      if (kout < p.K)
-        for (int c = ct * 128 + half * 64; c < min(p.C, ct * 128 + half * 64 + 64); ++c) wrow[c] = 0.f;
-    } else
-#pragma unroll 1
-    for (int j = 2 * half; j < 2 * half + 2; ++j) {
-      uint32_t v[32], u[32];
-      const uint32_t taddr = tmem_base + lane_addr + (uint32_t)(j * 32);
-      tmem_ld32(taddr, v);
-      tmem_ld32(taddr + 128u, u);
-      asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-      if (kout < p.K) {
-        const int c0 = ct * 128 + j * 32;
-#pragma unroll
-        for (int i = 0; i < 32; ++i)
-          if (c0 + i < p.C) wrow[c0 + i] = fmaf(__uint_as_float(u[i]), LO_UNSCALE, __uint_as_float(v[i])) * f1 * f2;
-      }
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+    return;
   }
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512) : "memory");
+  setmaxnreg_inc<232>();
+  const int c = wg - 1;                       // consumer warpgroup: dy block c (out-channels 64c .. 64c+63) and x block c
+  const int warp = tid >> 5, lane = tid & 31;
+  const int Ey = amax_exponent(p.amax_y), Ex = amax_exponent(p.amax_x);
+  const float sy = scale_up(Ey), sxs = scale_up(Ex);
+  // dy task: channel ch of block c, pixels 32 dh .. 32 dh + 31
+  const int ch = tid & 63, dh = tid >> 6;
+  const bool dy_valid = ((64 * c + ch) >> 5) < dy_boxes;
+  const uint32_t dy_raw = (uint32_t)((ch >> 5) * 2 + c) * WG_BLK, bl = (uint32_t)(ch & 31);
+  // x task: pixel row xp of block c, raw box xh (channels 32 xh .. 32 xh + 31 of the block)
+  const int xp = tid & 63, xh = tid >> 6;
+  const bool x_valid = 2 * c + xh < x_boxes;
+  const uint32_t xsw = (uint32_t)(xp & 7);
+  float bsum = 0.f;                           // sum of this thread's out-channel of dy over its pixels of the split (bias gradient)
+  float acc[64], cor[64];
+  int prev_s = 0;
+  for (int it = 0; it < num_iters; ++it) {
+    const int s = it % WG_STAGES;
+    const uint32_t ph = (uint32_t)(it / WG_STAGES) & 1u;
+    mbar_wait(full_bar(s), ph);
+    uint8_t* stp = smem + s * WG_STAGE_BYTES;
+    float dv[32];
+    if (dy_valid) {
+#pragma unroll
+      for (int j = 0; j < 32; ++j) {     // 16-byte chunk q of row `pix` sits at position q ^ (pix & 7)
+        const int pix = 32 * dh + j;
+        dv[j] = *reinterpret_cast<const float*>(stp + dy_raw + pix * 128 + ((((bl >> 2) ^ (uint32_t)pix) & 7u) << 4) + (bl & 3u) * 4);
+      }
+    }
+    uint8_t* x0 = stp + 4 * WG_BLK + c * WG_BLK + xp * 128;     // row xp of x_hi[c] (over the raw box of channels 64c .. 64c+31)
+    uint8_t* x1 = x0 + 2 * WG_BLK;                              // row xp of x_lo'[c]
+    float4 xv[8];
+    if (x_valid) {
+      const uint8_t* src = xh ? x1 : x0;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) xv[j] = *reinterpret_cast<const float4*>(src + ((j ^ xsw) << 4));
+    }
+    named_sync(1 + c, 128);                   // block c of both operands has been read
+    if (dy_valid) {
+      __half* dh_hi = reinterpret_cast<__half*>(stp + c * WG_BLK);
+      __half* dh_lo = reinterpret_cast<__half*>(stp + (2 + c) * WG_BLK);
+      float ssum = 0.f;
+#pragma unroll
+      for (int j = 0; j < 32; j += 2) {
+        ssum += dv[j] + dv[j + 1];
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int pix = 32 * dh + j + e;
+          const int off = pix * 64 + ((((ch >> 3) ^ pix) & 7) << 3) + (ch & 7);
+          split1(dv[j + e] * sy, dh_hi[off], dh_lo[off]);
+        }
+      }
+      bsum += ssum;
+    }
+    if (x_valid) {
+#pragma unroll
+      for (int m = 0; m < 4; ++m) {
+        const float4 u0 = xv[2 * m], u1 = xv[2 * m + 1];
+        uint4 hq, lq;
+        split2(u0.x * sxs, u0.y * sxs, hq.x, lq.x);
+        split2(u0.z * sxs, u0.w * sxs, hq.y, lq.y);
+        split2(u1.x * sxs, u1.y * sxs, hq.z, lq.z);
+        split2(u1.z * sxs, u1.w * sxs, hq.w, lq.w);
+        const uint32_t pos = (uint32_t)(((4 * xh + m) ^ xsw) << 4);
+        *reinterpret_cast<uint4*>(x0 + pos) = hq;
+        *reinterpret_cast<uint4*>(x1 + pos) = lq;
+      }
+    }
+    fence_proxy_async();
+    named_sync(3, 256);                       // both blocks of x are split (each warpgroup's B spans both)
+    const uint32_t st = sbase + s * WG_STAGE_BYTES;
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < WG_KPIX / 16; ++k) {     // 16 pixels per instruction = two 8-pixel groups (2 KB) further into every block
+      const uint64_t a_hi = desc_mn(st + c * WG_BLK + k * 2048, WG_BLK), a_lo = desc_mn(st + (2 + c) * WG_BLK + k * 2048, WG_BLK);
+      const uint64_t b_hi = desc_mn(st + 4 * WG_BLK + k * 2048, WG_BLK), b_lo = desc_mn(st + 6 * WG_BLK + k * 2048, WG_BLK);
+      const uint32_t first = (it > 0 || k > 0) ? 1u : 0u;
+      wgmma_f16_n128<1, 1>(acc, a_hi, b_hi, first);
+      wgmma_f16_n128<1, 1>(cor, a_hi, b_lo, first);
+      wgmma_f16_n128<1, 1>(cor, a_lo, b_hi, 1u);
+    }
+    wgmma_commit();
+    wgmma_wait<1>();
+    if (it > 0 && lane == 0) mbar_arrive(empty_bar(prev_s));
+    prev_s = s;
+  }
+  wgmma_wait<0>();
+  fence_regs(acc); fence_regs(cor);
+  if (dh) bsh[64 * c + ch] = bsum;
+  named_sync(3, 256);
+  if (!dh) {
+    bsum += bsh[64 * c + ch];
+    const int kout = kt * 128 + 64 * c + ch;
+    if (p.bias_ws && tap == 0 && ct == 0 && kout < p.K) p.bias_ws[(long long)blockIdx.y * p.K + kout] = bsum;   // 0 for an empty split
+  }
+  const float f1 = scale_dn(Ey), f2 = scale_dn(Ex);
+  const long long TC_ = (long long)T * p.C;
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    const int kout = kt * 128 + 64 * c + 16 * warp + (lane >> 2) + 8 * i;
+    if (kout >= p.K) continue;
+    float* wrow = p.ws + ((long long)blockIdx.y * p.K + kout) * TC_ + (long long)tap * p.C;
+#pragma unroll
+    for (int j = 0; j < 16; ++j)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int col = ct * 128 + 8 * j + 2 * (lane & 3) + e;
+        // an empty split accumulated nothing (the registers hold garbage): it contributes zeros
+        if (col < p.C) wrow[col] = num_iters ? fmaf(cor[4 * j + 2 * i + e], LO_UNSCALE, acc[4 * j + 2 * i + e]) * f1 * f2 : 0.f;
+      }
   }
 }
 
@@ -853,9 +536,9 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t,
                                   CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 EncodeTiledFn g_encode = nullptr;
 int g_tc_state = -1;  // -1 unknown, 0 unavailable, 1 ok
-int g_num_sms = 148;
+int g_num_sms = 132;   // H100 SXM; tc_init reads the device's count
 std::mutex g_tc_mutex;
-constexpr int PS_SMEM = PS_STAGES * (2 * A_BYTES + 2 * 128 * BK * 2) + 2048;
+constexpr int PS_SMEM = PS_STAGES * PS_STAGE_BYTES + 2048;
 constexpr int WG_SMEM = WG_STAGES * WG_STAGE_BYTES + 2048;
 
 // Row length (fp16 elements) of the packed weight tiles (dp_pack_conv_weight_tc): rows longer than 64 are zero-padded to a multiple of
@@ -869,14 +552,13 @@ int tc_init() {
   g_tc_state = 0;
   int dev = 0, major = 0;
   if (cudaGetDevice(&dev) != cudaSuccess) { (void)cudaGetLastError(); return 0; }
-  if (cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev) != cudaSuccess || major != 10) { (void)cudaGetLastError(); return 0; }
+  if (cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev) != cudaSuccess || major != 9) { (void)cudaGetLastError(); return 0; }
   void* fn = nullptr;
   cudaDriverEntryPointQueryResult qres;
   if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres) != cudaSuccess || !fn ||
       qres != cudaDriverEntryPointSuccess) { (void)cudaGetLastError(); return 0; }
   g_encode = (EncodeTiledFn)fn;
-  bool ok = cudaFuncSetAttribute(conv_tc_ps_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, PS_SMEM) == cudaSuccess;
-  ok = ok && cudaFuncSetAttribute(conv_tc_ps_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, PS_SMEM) == cudaSuccess;
+  bool ok = cudaFuncSetAttribute(conv_tc_ps_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, PS_SMEM) == cudaSuccess;
   ok = ok && cudaFuncSetAttribute(wgrad_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_SMEM) == cudaSuccess;
   cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev);
   if (!ok) { (void)cudaGetLastError(); return 0; }
@@ -997,8 +679,7 @@ int launch_tc(const float* act, long long ld_act, const uint32_t* amax_a, int Ni
     }
     const int work = total * p.ksplit;
     const int ctas = work < g_num_sms ? work : g_num_sms;
-    if (p.it_per_split >= PS_TS_MIN_STAGES) conv_tc_ps_kernel<true><<<ctas, PS_THREADS, PS_SMEM, st>>>(mA, mBh, mBl, p, tiles_m, total);
-    else conv_tc_ps_kernel<false><<<ctas, PS_THREADS, PS_SMEM, st>>>(mA, mBh, mBl, p, tiles_m, total);
+    conv_tc_ps_kernel<<<ctas, THREADS, PS_SMEM, st>>>(mA, mBh, mBl, p, tiles_m, total);
     if (p.ksplit > 1) {
       int rc = dp_check_launch();
       if (rc) return rc;
@@ -1011,11 +692,6 @@ int launch_tc(const float* act, long long ld_act, const uint32_t* amax_a, int Ni
   return dp_check_launch();
 }
 
-// one scaled fp32 value -> fp16 hi and lo' = (v - hi) * 2^11
-__device__ __forceinline__ void split1(float v, __half& h, __half& l) {
-  h = __float2half_rn(v);
-  l = __float2half_rn((v - __half2float(h)) * LO_SCALE);
-}
 __global__ void pack_tc_kernel(const float* __restrict__ w, int K, int C, int RS, int Cp, int Kp, __half* __restrict__ kc_hi,
                                __half* __restrict__ kc_lo, __half* __restrict__ ck_hi, __half* __restrict__ ck_lo,
                                const uint32_t* __restrict__ amax) {
@@ -1157,7 +833,7 @@ extern "C" int dp_split_h3(const float* x, int64_t ld, int64_t bs, int32_t batch
     const int pitch = (cols + 7) & ~7;
     const int vec = ((((uintptr_t)x) & 15) == 0 && ld % 4 == 0 && bs % 4 == 0) ? 1 : 0;
     long long blocks = ((long long)rows * (pitch >> 3) + 255) / 256;
-    if (blocks > 148 * 8) blocks = 148 * 8;
+    if (blocks > g_num_sms * 8) blocks = g_num_sms * 8;
     split_h3_rows_kernel<<<dim3((unsigned)blocks, (unsigned)batch), 256, 0, (cudaStream_t)stream>>>(x, ld, bs, rows, cols, pitch, vec, (__half*)hi,
                                                                                                 (__half*)lo, amax);
   } else {
@@ -1330,7 +1006,7 @@ int dp_conv2d_wgrad_tc(const dp_conv_args* a, dp_stream_t stream) {
   p.ws = a->workspace;
   const int k_tiles = (a->K + 127) / 128;
   dim3 grid((unsigned)(k_tiles * p.c_tiles * a->R * a->S), (unsigned)a->splits);
-  wgrad_tc_kernel<<<grid, WG_THREADS, WG_SMEM, (cudaStream_t)stream>>>(mDy, mX, p);
+  wgrad_tc_kernel<<<grid, THREADS, WG_SMEM, (cudaStream_t)stream>>>(mDy, mX, p);
   return dp_check_launch();
 }
 
@@ -1346,7 +1022,7 @@ extern "C" int dp_pack_conv_weight_tc(const float* w, int32_t K, int32_t C, int3
   const int Cp = wrow(C), Kp = wrow(K);
   long long total = (long long)R * S * ((long long)K * Cp > (long long)C * Kp ? (long long)K * Cp : (long long)C * Kp);
   int blocks = (int)((total + 255) / 256);
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > g_num_sms * 16) blocks = g_num_sms * 16;
   pack_tc_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(w, K, C, R * S, Cp, Kp, (__half*)kc_hi, (__half*)kc_lo, (__half*)ck_hi, (__half*)ck_lo,
                                                            amax_w);
   return dp_check_launch();

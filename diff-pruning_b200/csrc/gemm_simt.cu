@@ -5,7 +5,7 @@
 // loaders are compile-time "modes": plain strided (k-contiguous / m|n-contiguous) or an on-the-fly im2col
 // GATHER from an NHWC activation view, which turns the same kernel into conv fprop, dgrad and wgrad
 // (split-K over pixels, fixed-order reduce => deterministic).  This is the exact-fp32 path: every shape the
-// model can take after pruning runs here; the tcgen05 path (conv_tc.cu) takes over the big regular convs.
+// model can take after pruning runs here; the wgmma path (conv_tc.cu) takes over the big regular convs.
 #include "common.cuh"
 
 namespace {
@@ -501,7 +501,7 @@ extern "C" int dp_conv2d_wgrad_reduce(const dp_wgrad_reduce_args* a, dp_stream_t
   if (RS == 1 && a->C % 4 == 0 && ((((uintptr_t)a->workspace) | ((uintptr_t)a->dw) | ((uintptr_t)a->w)) & 15) == 0) {
     // flat tensor (every nn.Linear / 1x1 convolution: most of the 400 M LDM parameters): 4 elements per thread, grid-stride
     long long blocks = (kc / 4 + 255) / 256;
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > DP_NUM_SMS * 16) blocks = DP_NUM_SMS * 16;
     wgrad_reduce_flat4_kernel<<<(unsigned)(blocks < 1 ? 1 : blocks), 256, 0, st>>>(*a);
   } else {
     DP_REQUIRE(a->K <= 65535, DP_ERR_SHAPE);
@@ -526,7 +526,7 @@ extern "C" int dp_pack_conv_weight(const float* w, int32_t K, int32_t C, int32_t
   DP_REQUIRE(K > 0 && C > 0 && R > 0 && S > 0, DP_ERR_SHAPE);
   long long total = (long long)K * C * R * S;
   int blocks = (int)((total + 255) / 256);
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > DP_NUM_SMS * 16) blocks = DP_NUM_SMS * 16;
   pack_weight_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(w, K, C, R * S, w_ck, w_kc);
   return dp_check_launch();
 }

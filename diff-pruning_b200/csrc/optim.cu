@@ -112,7 +112,7 @@ extern "C" int dp_adam_clip_ema(const dp_adam_args* a, dp_stream_t stream) {
   k.w1 = (float)(1.0 - a->beta1); k.w2 = (float)(1.0 - a->beta2); k.beta2 = (float)a->beta2; k.eps = (float)a->eps;
   k.max_norm = (float)a->max_norm; k.ema_d = (float)a->ema_decay; k.ema_1md = (float)(1.0 - a->ema_decay);
   long long nb = (a->n + NT * 4 - 1) / (NT * 4);
-  if (nb > 148 * 16) nb = 148 * 16;
+  if (nb > DP_NUM_SMS * 16) nb = DP_NUM_SMS * 16;
   adam_kernel<<<(unsigned)nb, NT, 0, (cudaStream_t)stream>>>(*a, k);
   return dp_check_launch();
 }

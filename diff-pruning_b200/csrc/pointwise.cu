@@ -5,7 +5,7 @@
 
 namespace {
 constexpr int NT = 256;
-static inline int nblocks(long long n, int per_block, int cap = 148 * 32) {
+static inline int nblocks(long long n, int per_block, int cap = DP_NUM_SMS * 32) {
   long long b = (n + per_block - 1) / per_block;
   if (b < 1) b = 1;
   if (b > cap) b = cap;
@@ -288,13 +288,13 @@ extern "C" int dp_amax(const float* x, int64_t ld, int64_t rows, int32_t cols, u
   long long r = rows, c = cols;
   if (ld == cols) { c = r * c; r = 1; }                     // dense: one long row
   const int vec = ((((uintptr_t)x) & 15) == 0 && c % 4 == 0 && (r == 1 || ld % 4 == 0)) ? 1 : 0;
-  amax_kernel<<<nblocks(vec ? r * (c >> 2) : r * c, NT * 4, 148 * 8), NT, 0, (cudaStream_t)st>>>(x, ld, r, c, vec, slot);
+  amax_kernel<<<nblocks(vec ? r * (c >> 2) : r * c, NT * 4, DP_NUM_SMS * 8), NT, 0, (cudaStream_t)st>>>(x, ld, r, c, vec, slot);
   return dp_check_launch();
 }
 extern "C" int dp_zero_u32(uint32_t* p, int64_t n, dp_stream_t st) {
   DP_REQUIRE(p, DP_ERR_NULL);
   DP_REQUIRE(n > 0, DP_ERR_SHAPE);
-  zero_u32_kernel<<<nblocks(n, NT, 148), NT, 0, (cudaStream_t)st>>>(p, n);
+  zero_u32_kernel<<<nblocks(n, NT, DP_NUM_SMS), NT, 0, (cudaStream_t)st>>>(p, n);
   return dp_check_launch();
 }
 extern "C" int dp_silu_fwd(const float* x, float* y, int64_t n, dp_stream_t st) {

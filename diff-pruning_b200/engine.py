@@ -1,4 +1,4 @@
-"""Planned sm_100a executor for the UNet2DModel forward + backward (the Taylor-scoring / finetune hot path).
+"""Planned sm_90a executor for the UNet2DModel forward + backward (the Taylor-scoring / finetune hot path).
 
 Instead of dispatching ~1000 ATen ops per pass through autograd (SURVEY.md §3.1: ddpm_prune.py:100-102 ->
 unet_2d.py:219 -> autograd), the engine walks the module tree ONCE per (batch, resolution), lays every
@@ -32,15 +32,15 @@ _byref = C.byref
 Step = Callable[[int], None]
 
 
-_SM_COUNT = 148            # B200; the wgrad kernel runs one CTA per SM (192 KB of shared memory)
-_WGRAD_CTA_OVERHEAD = 8    # per-CTA prologue + pipeline fill + TMEM->workspace epilogue, in units of one 64-pixel stage
+_SM_COUNT = 132            # H100 SXM; the wgrad kernel runs one CTA per SM (192 KB of shared memory)
+_WGRAD_CTA_OVERHEAD = 8    # per-CTA prologue + pipeline fill + register->workspace epilogue, in units of one 64-pixel stage
 
 
 def _wgrad_splits(tiles, chunks, env=os.environ.get("DPB200_WGRAD_WAVES")):
     """Split-K factor of the tensor-core wgrad: grid = tiles x splits CTAs, each walking ceil(chunks / splits) pixel chunks.
-    One CTA per SM, so the launch runs in ceil(grid / 148) strict waves: pick the split count whose modelled time
+    One CTA per SM, so the launch runs in ceil(grid / 132) strict waves: pick the split count whose modelled time
     waves x (overhead + chunks per CTA) is smallest (ties: fewer splits = smaller workspace), so a grid never overshoots a
-    wave boundary by a few CTAs (592 -> 594 CTAs used to cost a fifth, almost empty, wave) and no trailing split is empty."""
+    wave boundary by a few CTAs (530 CTAs would cost a fifth, almost empty, wave) and no trailing split is empty."""
     max_waves = int(env) if env else 8
     hi = max(1, min(chunks, max(2, (max_waves * _SM_COUNT) // tiles)))
     best = None
@@ -129,7 +129,7 @@ class Plan:
         if compute not in ("fp32", "bf16"):
             raise ValueError(f"compute must be 'fp32' (3 x fp16 split, fp32-grade) or 'bf16' (single-pass tensor tier), got {compute!r}")
         if compute == "bf16" and not (torch.device(device).type == "cuda" and self.lib.dp_bf16_available()):
-            raise RuntimeError("diff_pruning_b200: the bf16 tensor tier needs an sm_100a device (no fallback)")
+            raise RuntimeError("diff_pruning_b200: the bf16 tensor tier needs an sm_90a device (no fallback)")
         # bf16 tier (ddpm_train.py --mixed_precision bf16 -> torch.autocast: conv / linear operands in bf16, everything else fp32):
         # eligible convolutions read bf16 operands (written by GroupNorm+SiLU directly, or by dp_cvt_bf16) on the kind::f16 kernels
         self.compute = compute
@@ -947,7 +947,7 @@ class Plan:
         self.conv(o, m.to_out[0].weight, m.to_out[0].bias, out, pad=0, residual=x if m.residual_connection else None)
 
     def _attn_core(self, q: View, k: View, v: View, o: View, sc: float):
-        """o = softmax(sc * q k^T) v per image over the H*W tokens (single head) and its backward: tcgen05 NT GEMMs when the token
+        """o = softmax(sc * q k^T) v per image over the H*W tokens (single head) and its backward: tensor-core NT GEMMs when the token
         count is a multiple of 128, the exact SIMT batched GEMM otherwise."""
         lib = self.lib
         N, H, W, inner = q.N, q.H, q.W, q.C

@@ -6,7 +6,7 @@ model_channels 192, channel_mult (1,2,3,5), 2 res blocks, attention at ds {2,4,8
 so `torch.manual_seed(s); UNetModel(**cfg)` reproduces the reference's parameters (incl. its zero-initialised output convolutions) and
 state-dict keys, and `torch_pruning`-style tools find real nn.Conv2d / nn.Linear / nn.GroupNorm / nn.LayerNorm leaves.
 
-On CUDA the forward (and, through autograd, the backward) is the planned sm_100a engine (engine.Plan._build_ldm); under
+On CUDA the forward (and, through autograd, the backward) is the planned sm_90a engine (engine.Plan._build_ldm); under
 models.trace_mode() the leaves run as torch ops (dependency tracing, host-side structure tests).  No CPU fallback otherwise.
 
 Not rebuilt: the AttentionBlock (non-transformer) variant, resblock_updown, scale-shift norm, num_classes label embedding, 1-D / 3-D.
@@ -266,7 +266,7 @@ class UNetModel(nn.Module):
             out = self._forward_traced(x, timesteps, context)
         else:
             if not x.is_cuda:
-                raise RuntimeError("diff_pruning_b200: the LDM UNetModel runs on the sm_100a CUDA engine only (CPU execution exists only under "
+                raise RuntimeError("diff_pruning_b200: the LDM UNetModel runs on the sm_90a CUDA engine only (CPU execution exists only under "
                                    "models.trace_mode()). No CPU fallback is provided.")
             from .engine import unet_apply
             out = unet_apply(self, x, timesteps, context=context)

@@ -11,7 +11,7 @@ reference, (ii) state dicts are interchangeable, (iii) torch_pruning-style tools
 nn.Conv2d / nn.Linear / nn.GroupNorm leaves and mutate them in place.
 
 Execution:
-  * CUDA tensors  -> the planned sm_100a engine (engine.py) behind one autograd node; the C-ABI
+  * CUDA tensors  -> the planned sm_90a engine (engine.py) behind one autograd node; the C-ABI
     library must be present, otherwise a RuntimeError is raised (no silent fallback).
   * ``with trace_mode():`` -> leaf-module-by-leaf-module execution with torch ops. This exists only
     for structure discovery (dependency tracing with forward hooks at batch 1, MAC counting,
@@ -480,7 +480,7 @@ class UNet2DModel(nn.Module):
         else:
             if not sample.is_cuda:
                 raise RuntimeError(
-                    "diff_pruning_b200: UNet2DModel runs on the sm_100a CUDA engine only; move the model and "
+                    "diff_pruning_b200: UNet2DModel runs on the sm_90a CUDA engine only; move the model and "
                     "inputs to a CUDA device (CPU execution exists only under models.trace_mode() for "
                     "dependency tracing). No CPU fallback is provided.")
             from .engine import unet_apply

@@ -1,4 +1,4 @@
-/* dpb200.h — C-ABI of libdpb200.so: the sm_100a device math behind the reference's Python API boundary.
+/* dpb200.h — C-ABI of libdpb200.so: the sm_90a (H100) device math behind the reference's Python API boundary.
  *
  * The reference (VainF/Diff-Pruning) has no FFI of its own: its hot path dispatches ATen ops from Python
  * (SURVEY.md §2.3).  Each entry point below replaces the ATen/cuDNN/cuBLAS op(s) the reference reaches from
@@ -39,7 +39,7 @@ const char* dp_strerror(int code);
 int dp_last_cuda_error(void);
 /* number of CUDA kernels this library has launched in this process (monotonic; for gpu_launches accounting) */
 int64_t dp_launch_count(void);
-/* 1 if the tcgen05/TMA tensor-core path is compiled in and usable on the current device, else 0 */
+/* 1 if the wgmma/TMA tensor-core path is compiled in and usable on the current device, else 0 */
 int dp_tc_available(void);
 
 /* ------------------------------------------------------------------------------------------------
@@ -114,7 +114,7 @@ int dp_conv2d_wgrad_reduce(const dp_wgrad_reduce_args* a, dp_stream_t stream);
 int dp_pack_conv_weight(const float* w_oihw, int32_t K, int32_t C, int32_t R, int32_t S, float* w_ck, float* w_kc,
                         dp_stream_t stream);
 
-/* Operands of the tcgen05 path (3 x fp16 split, fp32-grade).  With s = the power of two that brings the tensor's max|w| below 2^14:
+/* Operands of the wgmma path (3 x fp16 split, fp32-grade).  With s = the power of two that brings the tensor's max|w| below 2^14:
  *   hi = fp16(s*w), lo = fp16((s*w - hi) * 2^11), each in both K-major forms:
  *   kc_* [R*S][K][Cp] (fprop B operand, GEMM-K = C)   ck_* [R*S][C][Kp] (dgrad B operand, GEMM-K = K), where
  *   Cp = dp_tc_weight_row(C), Kp = dp_tc_weight_row(K) are the zero-padded row lengths in fp16 ELEMENTS: a multiple of 64 for rows
@@ -129,7 +129,7 @@ int dp_amax(const float* x, int64_t ld, int64_t rows, int32_t cols, uint32_t* sl
 int dp_zero_u32(uint32_t* p, int64_t n, dp_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
- * bf16 tensor tier (conv_bf16.cu): tcgen05.mma kind::f16 on BF16 operands, fp32 accumulation — what torch.autocast(bfloat16) makes of
+ * bf16 tensor tier (conv_bf16.cu): wgmma on BF16 operands, fp32 accumulation — what torch.autocast(bfloat16) makes of
  * aten::convolution / linear in the finetune step (ddpm_train.py:200-208,255-261 `--mixed_precision bf16`; BASELINE configs[3]).
  * Operands are bf16 NHWC views (pixel stride in ELEMENTS, a multiple of 8) produced by dp_cvt_bf16 or by dp_groupnorm_fwd's y_bf16
  * output; outputs (y, dx, the wgrad workspace) are fp32 exactly as in dp_conv_args, so bias / temb / residual epilogues, the
@@ -180,7 +180,7 @@ int dp_gemm_batched(const dp_gemm_args* a, dp_stream_t stream);
  *   C[b][m][n] = alpha * sum_k A[b][m][k] * B[b][n][k]          (both operands K-contiguous, "NT")
  * A: [batch][H*W][Kg] fp32 view (pixel stride ld_a) — the token grid is the image grid so a 128-token tile is a TMA box;
  * B: given pre-split (dp_split_h3) as fp16 b_hi/b_lo [batch][N][Kg8]; C: [batch][H*W][N] view (ldc); amax_a / amax_b: amax slots of
- * A and of the matrix B was split from.  Runs on the persistent tcgen05 kernel; returns DP_ERR_UNSUPPORTED when the shape is not
+ * A and of the matrix B was split from.  Runs on the persistent wgmma kernel; returns DP_ERR_UNSUPPORTED when the shape is not
  * eligible (H*W % 128, alignment) so the caller can fall back to dp_gemm_batched. */
 typedef struct dp_gemm_nt_args {
   int32_t batch, H, W, Kg, N;

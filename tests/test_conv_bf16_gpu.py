@@ -1,4 +1,4 @@
-"""bf16 tensor tier (conv_bf16.cu, tcgen05.mma kind::f16): op-level parity against a torch fp32 convolution of the SAME bf16-rounded
+"""bf16 tensor tier (conv_bf16.cu, bf16 wgmma): op-level parity against a torch fp32 convolution of the SAME bf16-rounded
 operands (products of bf16 values are exact in fp32, so only the fp32 accumulation order differs: tolerance 2e-5 on the tensor), and
 end to end — a finetune step of the engine in compute="bf16" against the oracle, with the tolerance bf16 operand rounding implies
 (the reference under `--mixed_precision bf16` = torch.autocast rounds conv OUTPUTS to bf16 as well, so its own distance to fp32 is the
@@ -22,7 +22,7 @@ def lib():
     from diff_pruning_b200 import _lib as L
     lib = L.load()
     if not lib.dp_bf16_available():
-        pytest.fail("bf16 tensor tier (tcgen05 kind::f16 / TMA) not available on this device: conv_bf16.cu must run on sm_100a")
+        pytest.fail("bf16 tensor tier (wgmma / TMA) not available on this device: conv_bf16.cu must run on sm_90a")
     return lib
 
 
@@ -151,7 +151,7 @@ def test_conv_bf16_fprop_dgrad_wgrad(lib, N, Cin, H, W, K, R, stride, pad):
         assert lib.dp_conv2d_wgrad_reduce(C.byref(ra), S()) == 0
         torch.cuda.synchronize()
         assert not torch.isnan(dw).any()
-        # the tensor core adds each K=16 product block into the fp32 TMEM accumulator with a truncating rounding; one CTA walking all
+        # the tensor core adds each K=16 product block into the fp32 accumulator with a truncating rounding; one CTA walking all
         # N*P*Q pixels (splits = 1, up to 65536 here = 4096 sequential accumulations) drifts by a few 1e-5 relative — the engine's
         # wave-aware split-K keeps the per-CTA reduction short; either way it is far below bf16 operand rounding (4e-3)
         assert rel_err(dw.cpu(), gw_ref) < (2e-5 if N * P * Q // splits <= 16384 else 2e-4), splits

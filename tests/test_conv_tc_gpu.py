@@ -1,6 +1,6 @@
-"""tcgen05/TMA implicit-GEMM convolution (conv_tc.cu) vs plain torch fp32 CPU convolution.
+"""wgmma/TMA implicit-GEMM convolution (conv_tc.cu) vs plain torch fp32 CPU convolution.
 Tolerance: the 3-product split (3 x fp16 on power-of-two-scaled operands for fprop / dgrad, 3xTF32 for wgrad) keeps 22 bits of every
-operand, fp32 accumulation in TMEM => 1.5e-5 on the tensor."""
+operand, fp32 accumulation in registers => 1.5e-5 on the tensor."""
 import ctypes as C
 import math
 
@@ -20,7 +20,7 @@ def lib():
     from diff_pruning_b200 import _lib as L
     lib = L.load()
     if not lib.dp_tc_available():
-        pytest.fail("tensor-core path (tcgen05/TMA) not available on this device: conv_tc.cu must run on sm_100a")
+        pytest.fail("tensor-core path (wgmma/TMA) not available on this device: conv_tc.cu must run on sm_90a")
     return lib
 
 
@@ -77,7 +77,7 @@ CASES = [
     (2, 192, 16, 16, 179, 1, 0, 1),     # pruned attention to_q: 192 -> 179 (odd N, output view with a 180-float pitch)
     (2, 179, 16, 16, 192, 1, 1, 0),     # pruned attention to_out: 179 -> 192 (odd GEMM-K: padded weight rows, 180-float pitch)
     (64, 358, 1, 1, 96, 1, 2, 0),       # pruned time_emb_proj: 358 -> 96
-    # >= 74 pairs of pixel tiles: the cta_group::2 pair kernel (conv_tc_pair_kernel)
+    # many pixel tiles: several persistent work items per CTA
     (32, 128, 32, 32, 128, 3, 0, 0),    # 256 tiles -> 128 supertiles, full N tile (64 weight rows per CTA)
     (151, 64, 8, 16, 128, 3, 0, 0),     # ODD tile count (151): the last pair's second tile lies past the batch (TMA zero fill, no store)
     (40, 256, 16, 16, 256, 3, 0, 0),    # two N tiles x 80 pixel-tile pairs
@@ -189,7 +189,7 @@ def test_conv_tc_fprop_dgrad(lib, N, Cin, H, W, K, R, ldx, ldy):
     assert rel_err(nchw(gxb[..., ldx:]), 2 * xr.grad) < 1.5e-5
     # wgrad (MN-major operands, both split in-kernel), deterministic split-K + reduce into dW (+=)
     pix_chunks = max(1, N * H * W // 64)
-    # the tensor core adds every K=8 product block into the fp32 TMEM accumulator with a truncating rounding, so ONE CTA walking tens of
+    # the tensor core adds every K-block of products into the fp32 accumulator with a truncating rounding, so ONE CTA walking tens of
     # thousands of pixels drifts by a few 1e-5 (7.5e-5 at 32768 pixels); the engine's wave-aware split-K keeps a CTA at <= 8192 pixels and
     # so do the large cases here (the small ones keep their 1 / 3 / 7-way splits incl. the trailing EMPTY split of 7 over 16 chunks)
     base = max(1, -(-(N * H * W) // 8192))
@@ -315,7 +315,7 @@ def test_stride2_fprop_wgrad_tc(lib, N, Cin, H, K, pad):
         assert (N, Cin, H, K, pad) not in {(8, 256, 8, 256, 0), (4, 128, 8, 96, 0)}
     chunks = max(1, N * P * P // 64)
     sdy = amax_slot(lib, gyd)
-    base = max(1, -(-(N * P * P) // 2048))       # keep a CTA's pixel chain short enough for the 1.5e-5 bound (TMEM accumulation truncates)
+    base = max(1, -(-(N * P * P) // 2048))       # keep a CTA's pixel chain short enough for the 1.5e-5 bound (tensor-core accumulation truncates)
     for splits in sorted({base, min(3 * base, chunks)}):
         ws = torch.full((splits * K * 9 * Cin,), float("nan"), device="cuda")
         wg = L.ConvArgs()

@@ -142,7 +142,7 @@ def test_planner_fuses_qkv_and_moves_groupnorm_param_grads_off_the_chain():
 
     class P(engine.Plan):
         def _build(self):
-            self.tc = True          # what dp_tc_available() answers on an sm_100a device
+            self.tc = True          # what dp_tc_available() answers on an sm_90a device
             return super()._build()
 
     torch.manual_seed(0)

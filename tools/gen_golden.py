@@ -1,8 +1,8 @@
 #!/usr/bin/env python
-"""Generate tests/golden/* by importing the UNMODIFIED reference (read-only /root/reference).
+"""Generate tests/golden/* by importing the UNMODIFIED reference (a read-only checkout named by DPB200_REFERENCE).
 
-Run in the build container only (the reference does not exist on the GPU box):
-    python tools/gen_golden.py [--skip-cfg1]
+Needs the reference checkout and CPUs only:
+    DPB200_REFERENCE=<checkout> python tools/gen_golden.py [--skip-cfg1] [--only NAME]
 Outputs (all small, committed):
     tests/golden/tiny_unet.pt      TINY config: inputs, output, loss, all grads after 1 pass (B=2)
     tests/golden/blocks.pt         one ResnetBlock2D (with shortcut) and one Attention: in/out/grads

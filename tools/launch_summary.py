@@ -20,14 +20,14 @@ for row in csv.DictReader(lines):
                 "gemm_simt<%s,%s> (attention batched GEMM)" % m.groups())
     m = re.search(r"conv_tc_kernel<(\d+)>", row["Kernel Name"])
     if m:
-        name = "conv_tc_kernel<BN=%s> (tcgen05 3xTF32 fprop/dgrad)" % m.group(1)
+        name = "conv_tc_kernel<BN=%s> (3xTF32 fprop/dgrad)" % m.group(1)
     m = re.search(r"wgrad_tc_kernel", row["Kernel Name"])
     if m:
-        name = "wgrad_tc_kernel (tcgen05 kind::f16, 3-product fp16 split: wgrad)"
-    for kn, label in (("conv_tc_ps_kernel", "conv_tc_ps_kernel (tcgen05 kind::f16, 3-product fp16 split: fprop/dgrad/NT GEMM, persistent)"),
-                      ("conv_tc_ts_kernel", "conv_tc_ts_kernel<64> (tcgen05 3xTF32 fprop/dgrad, <= 64 channels)"),
-                      ("conv_bf16_kernel", "conv_bf16_kernel (tcgen05 kind::f16 fprop/dgrad, persistent)"),
-                      ("wgrad_bf16_kernel", "wgrad_bf16_kernel (tcgen05 kind::f16 wgrad)")):
+        name = "wgrad_tc_kernel (fp16 wgmma, 3-product fp16 split: wgrad)"
+    for kn, label in (("conv_tc_ps_kernel", "conv_tc_ps_kernel (fp16 wgmma, 3-product fp16 split: fprop/dgrad/NT GEMM, persistent)"),
+                      ("conv_tc_ts_kernel", "conv_tc_ts_kernel<64> (3xTF32 fprop/dgrad, <= 64 channels)"),
+                      ("conv_bf16_kernel", "conv_bf16_kernel (bf16 wgmma fprop/dgrad, persistent)"),
+                      ("wgrad_bf16_kernel", "wgrad_bf16_kernel (bf16 wgmma wgrad)")):
         if kn in row["Kernel Name"]:
             name = label
     agg[name][0] += 1; agg[name][1] += v; tot += v

@@ -10,7 +10,7 @@ import types
 
 import torch  # noqa: F401  (must precede the matplotlib stub)
 
-REF = os.environ.get("DPB200_REFERENCE", "/root/reference")
+REF = os.environ["DPB200_REFERENCE"]   # path of the reference checkout
 
 
 def install():
