@@ -18,8 +18,8 @@
 //                         warpgroup splits its 64 rows of the raw fp32 A boxes IN PLACE into fp16 hi | lo' tiles, B = pre-split fp16
 //                         weights by TMA, 3 x 64 KB stages
 //   splitk_epilogue_kernel  fixed-order sum of the K splits + the epilogue (small-M launches)
-//   wgrad_tc_kernel       weight gradient: dY and X both split in place in shared memory, both MN-major, 64-pixel stages, split-K
-//                         over pixels
+//   wgrad_tc_kernel       weight gradient: dY^T split in registers (wgmma A from registers), X split in place in shared memory
+//                         (MN-major B), 64-pixel stages, split-K over pixels
 //   pack / split / transpose helpers; dp_gemm_nt_tc runs the attention GEMMs on the persistent kernel.
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -339,10 +339,11 @@ __global__ void __launch_bounds__(256) splitk_epilogue_kernel(const TcParams p, 
 // ------------------------------------------------------------------------------------------------ wgrad
 // dW[k][tap][c] = sum_pixels dy[pix][k] * x[pix @ tap][c]: M = out-channels (128 per tile), N = in-channels of one tap (128 per tile),
 // GEMM-K = pixels, 64 per pipeline stage.  Both operands are pixel-major fp32 activations, i.e. MN-major for this product.
-// A stage holds 8 raw TMA boxes [64 px][32 ch]: dy in [0, 32 KB), x in [32 KB, 64 KB); the boxes of channels [64j, 64j+32) and
-// [64j+32, 64j+64) land where the fp16 blocks hi[j] and lo'[j] will live ([hi0 | hi1 | lo0 | lo1], MN-major SWIZZLE_128B: LBO = 8 KB
-// between 64-channel blocks).  Consumer warpgroup c splits block c of both in place (dy: thread = channel, which also sums the bias
-// gradient; x: thread = pixel row), then main += dy_hi[c] x_hi, corr += dy_hi[c] x_lo' + dy_lo'[c] x_hi.
+// A stage holds 8 raw TMA boxes [64 px][32 ch]: dy in [0, 32 KB), x in [32 KB, 64 KB); the x boxes of channels [64j, 64j+32) and
+// [64j+32, 64j+64) land where the fp16 blocks x_hi[j] and x_lo'[j] will live ([hi0 | hi1 | lo0 | lo1], MN-major SWIZZLE_128B: LBO = 8 KB
+// between 64-channel blocks).  Consumer warpgroup c splits x block c in place (thread = pixel row) and reads its 64 out-channels of dy
+// straight into wgmma A fragments, split in registers (dy is never written back; the fragment rows also sum the bias gradient), then
+// main += dy_hi[c] x_hi, corr += dy_hi[c] x_lo' + dy_lo'[c] x_hi.
 // grid = (k tiles * c tiles * taps, splits): split z covers pixel chunks [z*cps, (z+1)*cps) and writes its partial
 // tile to workspace[z][k][tap*C + c]; dp_conv2d_wgrad_reduce sums splits in fixed order (deterministic).
 struct WgParams {
@@ -370,7 +371,6 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap mapDy, const __grid_constant
   const uint32_t bar0 = sbase + WG_STAGES * WG_STAGE_BYTES;
   auto full_bar = [&](int s) { return bar0 + 8u * s; };
   auto empty_bar = [&](int s) { return bar0 + 8u * (WG_STAGES + s); };
-  float* bsh = reinterpret_cast<float*>(smem + WG_STAGES * WG_STAGE_BYTES + 8 * 2 * WG_STAGES);   // 128 floats: the bias sums' halves meet here
   const int wg = threadIdx.x >> 7, tid = threadIdx.x & 127;
   if (threadIdx.x == 0) {
     for (int s = 0; s < WG_STAGES; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 8); }
@@ -392,7 +392,7 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap mapDy, const __grid_constant
   const int dy_boxes = min(4, (p.K - kt * 128 + 31) >> 5), x_boxes = min(4, (p.C - ct * 128 + 31) >> 5);
 
   if (wg == 0) {
-    setmaxnreg_dec<40>();
+    setmaxnreg_dec<24>();      // the TMA loop fits in 24: consumers get 240 (2 x 32 dy fragments + 128 accumulators + the x split)
     if (threadIdx.x == 0) {
       prefetch_map(&mapDy); prefetch_map(&mapX);
       for (int it = 0; it < num_iters; ++it) {
@@ -417,35 +417,32 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap mapDy, const __grid_constant
     }
     return;
   }
-  setmaxnreg_inc<232>();
+  setmaxnreg_inc<240>();
   const int c = wg - 1;                       // consumer warpgroup: dy block c (out-channels 64c .. 64c+63) and x block c
   const int warp = tid >> 5, lane = tid & 31;
   const int Ey = amax_exponent(p.amax_y), Ex = amax_exponent(p.amax_x);
   const float sy = scale_up(Ey), sxs = scale_up(Ex);
-  // dy task: channel ch of block c, pixels 32 dh .. 32 dh + 31
-  const int ch = tid & 63, dh = tid >> 6;
-  const bool dy_valid = ((64 * c + ch) >> 5) < dy_boxes;
-  const uint32_t dy_raw = (uint32_t)((ch >> 5) * 2 + c) * WG_BLK, bl = (uint32_t)(ch & 31);
+  // dy^T fragment (A from registers): out-channel rows 16 warp + lane/4 (+8) of block c, pixel pairs 2 (lane%4) + {0, 1} (+8) of each
+  // 16-pixel step.  Both rows lie in raw box 2c + warp/2 (slot (warp/2) * 2 + c).  Pixel p's 16-byte chunk j sits at j ^ (p & 7), and
+  // p & 7 = 2 (lane%4) + e for every step: the per-pixel loads of a warp are bank-conflict free
+  const bool dy_valid = 2 * c + (warp >> 1) < dy_boxes;
+  // address of (row, pixel 0) in a stage; row + 8 flips chunk bit 1 (XOR 32 B), pixel + 1 flips row bit 0 and chunk bit 0 (XOR 144 B)
+  const uint32_t cb = (uint32_t)(16 * (warp & 1) + (lane >> 2)), pe = (uint32_t)(2 * (lane & 3));
+  const uint32_t dy_off = (uint32_t)((warp >> 1) * 2 + c) * WG_BLK + pe * 128 + (((cb >> 2) ^ pe) << 4) + (cb & 3) * 4;
   // x task: pixel row xp of block c, raw box xh (channels 32 xh .. 32 xh + 31 of the block)
   const int xp = tid & 63, xh = tid >> 6;
   const bool x_valid = 2 * c + xh < x_boxes;
   const uint32_t xsw = (uint32_t)(xp & 7);
-  float bsum = 0.f;                           // sum of this thread's out-channel of dy over its pixels of the split (bias gradient)
+  float bsum[2] = {0.f, 0.f};                 // sums of this thread's pixels of its two out-channel rows over the split (bias gradient)
   float acc[64], cor[64];
   int prev_s = 0;
-  for (int it = 0; it < num_iters; ++it) {
+  // One stage: x block c split in place (B, both warpgroups read both blocks), dy^T fragments of four 16-pixel steps split into
+  // fah / fal, then 12 MMAs.  The MMAs of the stage before still read the other fragment set, so stages alternate between two sets.
+  auto stage = [&](uint32_t (&fah)[4][4], uint32_t (&fal)[4][4], const int it) {
     const int s = it % WG_STAGES;
     const uint32_t ph = (uint32_t)(it / WG_STAGES) & 1u;
     mbar_wait(full_bar(s), ph);
     uint8_t* stp = smem + s * WG_STAGE_BYTES;
-    float dv[32];
-    if (dy_valid) {
-#pragma unroll
-      for (int j = 0; j < 32; ++j) {     // 16-byte chunk q of row `pix` sits at position q ^ (pix & 7)
-        const int pix = 32 * dh + j;
-        dv[j] = *reinterpret_cast<const float*>(stp + dy_raw + pix * 128 + ((((bl >> 2) ^ (uint32_t)pix) & 7u) << 4) + (bl & 3u) * 4);
-      }
-    }
     uint8_t* x0 = stp + 4 * WG_BLK + c * WG_BLK + xp * 128;     // row xp of x_hi[c] (over the raw box of channels 64c .. 64c+31)
     uint8_t* x1 = x0 + 2 * WG_BLK;                              // row xp of x_lo'[c]
     float4 xv[8];
@@ -454,23 +451,7 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap mapDy, const __grid_constant
 #pragma unroll
       for (int j = 0; j < 8; ++j) xv[j] = *reinterpret_cast<const float4*>(src + ((j ^ xsw) << 4));
     }
-    named_sync(1 + c, 128);                   // block c of both operands has been read
-    if (dy_valid) {
-      __half* dh_hi = reinterpret_cast<__half*>(stp + c * WG_BLK);
-      __half* dh_lo = reinterpret_cast<__half*>(stp + (2 + c) * WG_BLK);
-      float ssum = 0.f;
-#pragma unroll
-      for (int j = 0; j < 32; j += 2) {
-        ssum += dv[j] + dv[j + 1];
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const int pix = 32 * dh + j + e;
-          const int off = pix * 64 + ((((ch >> 3) ^ pix) & 7) << 3) + (ch & 7);
-          split1(dv[j + e] * sy, dh_hi[off], dh_lo[off]);
-        }
-      }
-      bsum += ssum;
-    }
+    named_sync(1 + c, 128);                   // block c of x has been read
     if (x_valid) {
 #pragma unroll
       for (int m = 0; m < 4; ++m) {
@@ -487,30 +468,53 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap mapDy, const __grid_constant
     }
     fence_proxy_async();
     named_sync(3, 256);                       // both blocks of x are split (each warpgroup's B spans both)
+    if (dy_valid) {
+#pragma unroll
+      for (int k = 0; k < WG_KPIX / 16; ++k)
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {          // fragment register q: row +8 (q & 1), pixels +8 (q >> 1)
+          const uint8_t* d = stp + (16 * k + 8 * (q >> 1)) * 128;
+          const float v0 = *reinterpret_cast<const float*>(d + (dy_off ^ (32u * (q & 1))));
+          const float v1 = *reinterpret_cast<const float*>(d + (dy_off ^ (32u * (q & 1) + 144u)));
+          bsum[q & 1] += v0 + v1;
+          split2(v0 * sy, v1 * sy, fah[k][q], fal[k][q]);
+        }
+    } else {     // channels past the last box: rows that are never stored
+#pragma unroll
+      for (int k = 0; k < WG_KPIX / 16; ++k)
+#pragma unroll
+        for (int q = 0; q < 4; ++q) fah[k][q] = fal[k][q] = 0u;
+    }
     const uint32_t st = sbase + s * WG_STAGE_BYTES;
     wgmma_fence();
 #pragma unroll
     for (int k = 0; k < WG_KPIX / 16; ++k) {     // 16 pixels per instruction = two 8-pixel groups (2 KB) further into every block
-      const uint64_t a_hi = desc_mn(st + c * WG_BLK + k * 2048, WG_BLK), a_lo = desc_mn(st + (2 + c) * WG_BLK + k * 2048, WG_BLK);
       const uint64_t b_hi = desc_mn(st + 4 * WG_BLK + k * 2048, WG_BLK), b_lo = desc_mn(st + 6 * WG_BLK + k * 2048, WG_BLK);
       const uint32_t first = (it > 0 || k > 0) ? 1u : 0u;
-      wgmma_f16_n128<1, 1>(acc, a_hi, b_hi, first);
-      wgmma_f16_n128<1, 1>(cor, a_hi, b_lo, first);
-      wgmma_f16_n128<1, 1>(cor, a_lo, b_hi, 1u);
+      wgmma_f16_n128_rs<1>(acc, fah[k], b_hi, first);
+      wgmma_f16_n128_rs<1>(cor, fah[k], b_lo, first);
+      wgmma_f16_n128_rs<1>(cor, fal[k], b_hi, 1u);
     }
     wgmma_commit();
     wgmma_wait<1>();
     if (it > 0 && lane == 0) mbar_arrive(empty_bar(prev_s));
     prev_s = s;
+  };
+  // the odd tail stays outside the loop: on every path a set is rewritten only after the group that read it has retired
+  uint32_t fah0[4][4], fal0[4][4], fah1[4][4], fal1[4][4];
+  int it = 0;
+  for (; it + 1 < num_iters; it += 2) {
+    stage(fah0, fal0, it);
+    stage(fah1, fal1, it + 1);
   }
+  if (it < num_iters) stage(fah0, fal0, it);
   wgmma_wait<0>();
   fence_regs(acc); fence_regs(cor);
-  if (dh) bsh[64 * c + ch] = bsum;
-  named_sync(3, 256);
-  if (!dh) {
-    bsum += bsh[64 * c + ch];
-    const int kout = kt * 128 + 64 * c + ch;
-    if (p.bias_ws && tap == 0 && ct == 0 && kout < p.K) p.bias_ws[(long long)blockIdx.y * p.K + kout] = bsum;   // 0 for an empty split
+  // the four lanes of a row hold its pixel columns: fixed-order butterfly, every lane ends with the row's sum
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    bsum[i] += __shfl_xor_sync(0xffffffffu, bsum[i], 1);
+    bsum[i] += __shfl_xor_sync(0xffffffffu, bsum[i], 2);
   }
   const float f1 = scale_dn(Ey), f2 = scale_dn(Ex);
   const long long TC_ = (long long)T * p.C;
@@ -518,6 +522,7 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap mapDy, const __grid_constant
   for (int i = 0; i < 2; ++i) {
     const int kout = kt * 128 + 64 * c + 16 * warp + (lane >> 2) + 8 * i;
     if (kout >= p.K) continue;
+    if (p.bias_ws && tap == 0 && ct == 0 && (lane & 3) == 0) p.bias_ws[(long long)blockIdx.y * p.K + kout] = bsum[i];   // 0 for an empty split
     float* wrow = p.ws + ((long long)blockIdx.y * p.K + kout) * TC_ + (long long)tap * p.C;
 #pragma unroll
     for (int j = 0; j < 16; ++j)

@@ -65,6 +65,23 @@ __device__ __forceinline__ void wgmma_f16_n128(float (&d)[64], uint64_t a, uint6
       : DP_F32(0), DP_F32(32)
       : "l"(a), "l"(b), "r"(acc), "n"(TA), "n"(TB));
 }
+// The same product with A(64 x 16) from registers.
+// a[] is the thread's fragment of packed fp16 pairs (low half = lower k), warp w, lane l: a[0] = row 16w + l/4, k 2(l%4) + {0,1};
+// a[1] = row + 8;  a[2] = k + 8;  a[3] = row + 8, k + 8.  The registers must stay unchanged until the wgmma group that reads them
+// has retired.  TB = 1: B is MN-major (the register form has no A transpose).
+template <int TB>
+__device__ __forceinline__ void wgmma_f16_n128_rs(float (&d)[64], const uint32_t (&a)[4], uint64_t b, uint32_t acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %69, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "{%64, %65, %66, %67}, %68, p, 1, 1, %70;\n\t}"
+      : DP_F32(0), DP_F32(32)
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(acc), "n"(TB));
+}
 template <int TA, int TB>
 __device__ __forceinline__ void wgmma_bf16_n64(float (&d)[32], uint64_t a, uint64_t b, uint32_t acc) {
   asm volatile(
