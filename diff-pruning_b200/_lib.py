@@ -118,6 +118,10 @@ _SIGS = {
     "dp_adam_clip_ema": (C.c_int, [C.POINTER(AdamArgs), vp]),
     "dp_ddim_step": (C.c_int, [vp, vp, vp, vp, i64, f32, f32, f32, f32, f32, f32, vp]),
     "dp_scale": (C.c_int, [vp, i64, f32, vp]),
+    "dp_fid_input": (C.c_int, [vp, i32, i32, i32, i32, i32, vp, i64, i32, i32, i32, i32, vp, vp]),
+    "dp_pool3x3": (C.c_int, [vp, i64, vp, i64, i32, i32, i32, i32, i32, i32, i32, vp, vp]),
+    "dp_global_mean": (C.c_int, [vp, i64, vp, i64, i32, i32, i32, i32, vp]),
+    "dp_feature_moments": (C.c_int, [vp, i64, i64, i32, vp, vp, vp, vp]),
 }
 EXPORTS = tuple(_SIGS)
 

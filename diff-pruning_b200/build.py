@@ -8,7 +8,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libdpb200.so")
-SOURCES = ["api.cu", "gemm_simt.cu", "norm.cu", "pointwise.cu", "optim.cu", "conv_tc.cu", "conv_bf16.cu"]
+SOURCES = ["api.cu", "gemm_simt.cu", "norm.cu", "pointwise.cu", "optim.cu", "conv_tc.cu", "conv_bf16.cu", "fid.cu"]
 
 
 def _newer(src_paths, target):

@@ -9,6 +9,7 @@ int dp_conv2d_dgrad_simt(const dp_conv_args*, dp_stream_t);
 int dp_conv2d_wgrad_simt(const dp_conv_args*, dp_stream_t);
 #ifdef DPB200_HAVE_TC
 int dp_conv2d_fprop_tc(const dp_conv_args*, dp_stream_t);   // returns DP_ERR_UNSUPPORTED when the shape is not eligible
+int dp_conv2d_fprop_tc_any(const dp_conv_args*, dp_stream_t);   // general geometry (DP_CONV_ANY_GEOMETRY); same contract
 int dp_conv2d_dgrad_tc(const dp_conv_args*, dp_stream_t);
 int dp_conv2d_wgrad_tc(const dp_conv_args*, dp_stream_t);
 int dp_tc_runtime_ok();
@@ -43,6 +44,10 @@ extern "C" int dp_conv2d_fprop(const dp_conv_args* a, dp_stream_t s) {
   if (a && !(a->flags & DP_CONV_FORCE_SIMT)) {
     int rc = dp_conv2d_fprop_tc(a, s);
     if (rc != DP_ERR_UNSUPPORTED) return rc;
+    if (a->flags & DP_CONV_ANY_GEOMETRY) {
+      rc = dp_conv2d_fprop_tc_any(a, s);
+      if (rc != DP_ERR_UNSUPPORTED) return rc;
+    }
   }
 #endif
   return dp_conv2d_fprop_simt(a, s);

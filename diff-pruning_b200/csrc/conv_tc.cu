@@ -59,6 +59,13 @@ struct TcParams {
   // (row = tile_m * 128 + tile row, pitch ws_ld); splitk_epilogue_kernel sums the splits in fixed order and applies the epilogue
   int ksplit, it_per_split;
   float* ws; long long ws_split_stride; int ws_ld;
+  // general-geometry fprop (conv_tc_ps_kernel<true>): the M tiles are 128 consecutive flattened output pixels m = (n*P + p)*Q + q of an
+  // [N][P][Q] grid (the launcher sets Nimg = Ho = 1, Wo = M, bw = 128, so the epilogue maps row -> m = tile_m*128 + row), and the producer
+  // warpgroup gathers each stage's A rows from the NHWC input x [N][H][W][ldx] with cp.async: taps walked arithmetically (r, s) = (tap / S,
+  // tap % S), padding and tails as zero fill.  relu: y = max(y, 0) after every epilogue term (DP_CONV_RELU)
+  const float* gx; long long gldx;
+  int gH, gW, gC, gQ, gPQ, gS, gstride, gpad_t, gpad_l, gM;
+  int relu;
 };
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -88,6 +95,13 @@ __device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* map
       "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
       ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
       : "memory");
+}
+// 16-byte cp.async with zero fill past src_bytes (0 = nothing read), and the mbarrier arrival that fires when this thread's copies land
+__device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, uint32_t src_bytes) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(src_bytes) : "memory");
+}
+__device__ __forceinline__ void cp_async_mbar_arrive(uint32_t bar) {
+  asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(bar) : "memory");
 }
 __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, int c2) {
   asm volatile(
@@ -126,6 +140,7 @@ constexpr int PS_STAGES = 3, PS_BN = 128;
 constexpr int PS_B_BYTES = PS_BN * BK * 2;
 constexpr int PS_STAGE_BYTES = 2 * A_BYTES + 2 * PS_B_BYTES;
 
+template <bool ANY>
 __global__ void __launch_bounds__(THREADS, 1)
 conv_tc_ps_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapBh,
                   const __grid_constant__ CUtensorMap mapBl, const TcParams p, const int tiles_m, const int total_tiles) {
@@ -140,7 +155,8 @@ conv_tc_ps_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constan
   auto empty_bar = [&](int s) { return bar0 + 8u * (PS_STAGES + s); };
   const int wg = threadIdx.x >> 7, tid = threadIdx.x & 127;
   if (threadIdx.x == 0) {
-    for (int s = 0; s < PS_STAGES; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 8); }   // one arrival per consumer warp
+    // full: the TMA thread's expect_tx (+ one cp.async arrival per gathering producer thread); empty: one arrival per consumer warp
+    for (int s = 0; s < PS_STAGES; ++s) { mbar_init(full_bar(s), ANY ? 1 + 128 : 1); mbar_init(empty_bar(s), 8); }
     mbar_init_fence();
   }
   __syncthreads();
@@ -157,6 +173,45 @@ conv_tc_ps_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constan
 
   if (wg == 0) {
     setmaxnreg_dec<40>();
+    if constexpr (ANY) {
+      // thread t gathers A row t of every stage: 64 fp32 channels of one input pixel, 16 x 16 bytes, into the two raw boxes at the
+      // 128-byte-swizzled positions TMA would have used (chunk j of row t at j ^ (t & 7)), so the consumers are unchanged
+      const int t = threadIdx.x;
+      if (t == 0) { prefetch_map(&mapBh); prefetch_map(&mapBl); }
+      const uint32_t sw = (uint32_t)(t & 7);
+      uint32_t g = 0;
+      for (int wi = blockIdx.x; wi < total_work; wi += gridDim.x) {
+        const int tile = wi % total_tiles, it0 = (wi / total_tiles) * p.it_per_split, it1 = min(iters_per_tile, it0 + p.it_per_split);
+        const int nblk = tile / tiles_m, m = (tile - nblk * tiles_m) * BM + t;
+        const bool mv = m < p.gM;
+        const int n = mv ? m / p.gPQ : 0, rem = m - n * p.gPQ, pq = rem / p.gQ;
+        const int hb = pq * p.gstride - p.gpad_t, wb = (rem - pq * p.gQ) * p.gstride - p.gpad_l;
+        const float* xn = p.gx + (long long)n * p.gH * p.gW * p.gldx;
+        for (int it = it0; it < it1; ++it, ++g) {
+          const int s = g % PS_STAGES;
+          const uint32_t ph = (g / PS_STAGES) & 1u;
+          mbar_wait(empty_bar(s), ph ^ 1u);
+          const int tap = it / p.kchunks, kc = it - tap * p.kchunks;
+          const int r = tap / p.gS, h = hb + r, w = wb + (tap - r * p.gS);
+          const uint32_t st = sbase + s * PS_STAGE_BYTES;
+          if (t == 0) {
+            mbar_expect_tx(full_bar(s), 2 * PS_B_BYTES);
+            tma_load_3d(st + 2 * A_BYTES, &mapBh, full_bar(s), kc * BK, nblk * PS_BN, tap);
+            tma_load_3d(st + 2 * A_BYTES + PS_B_BYTES, &mapBl, full_bar(s), kc * BK, nblk * PS_BN, tap);
+          }
+          const bool v = mv && h >= 0 && h < p.gH && w >= 0 && w < p.gW;
+          const int cleft = v ? p.gC - kc * BK : 0;       // valid channels from the stage's first one
+          const float* src = v ? xn + ((long long)h * p.gW + w) * p.gldx + kc * BK : p.gx;
+#pragma unroll
+          for (int j = 0; j < 16; ++j) {
+            const int nb = min(max(cleft - 4 * j, 0), 4) * 4;
+            cp_async16(st + (j >> 3) * A_BYTES + t * 128 + ((((uint32_t)j & 7u) ^ sw) << 4), nb ? src + 4 * j : p.gx, (uint32_t)nb);
+          }
+          cp_async_mbar_arrive(full_bar(s));
+        }
+      }
+      return;
+    }
     if (threadIdx.x == 0) {
       prefetch_map(&mapA); prefetch_map(&mapBh); prefetch_map(&mapBl);
       uint32_t g = 0;
@@ -259,6 +314,7 @@ conv_tc_ps_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constan
       const int w_l = row % p.bw, h_l = (row / p.bw) % p.bh, n_l = row / (p.bw * p.bh);
       const int img = n0 + n_l;
       if (img >= p.Nimg) continue;
+      if constexpr (ANY) { if (q0 + w_l >= p.Wo) continue; }   // the tail of the last flattened tile
       const long long m = ((long long)img * p.Ho + ((p0 + h_l) * p.os + p.oa)) * p.Wo + ((q0 + w_l) * p.os + p.ob);
       float* yrow = p.y + m * p.ldy;
       const float* rrow = p.residual ? p.residual + m * p.ld_res : nullptr;
@@ -273,6 +329,7 @@ conv_tc_ps_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constan
           if (rrow) { const float2 t = __ldg(reinterpret_cast<const float2*>(rrow + col)); o[0] += t.x; o[1] += t.y; }
           float2* dst = reinterpret_cast<float2*>(yrow + col);
           if (p.accumulate) { const float2 t = *dst; o[0] += t.x; o[1] += t.y; }
+          if constexpr (ANY) { if (p.relu) { o[0] = fmaxf(o[0], 0.f); o[1] = fmaxf(o[1], 0.f); } }
           *dst = make_float2(o[0], o[1]);
           amax = fmaxf(amax, fmaxf(fabsf(o[0]), fabsf(o[1])));
         } else {
@@ -285,6 +342,7 @@ conv_tc_ps_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constan
               if (arow2) ov += __ldg(arow2 + cc);
               if (rrow) ov += __ldg(rrow + cc);
               if (p.accumulate) ov += yrow[cc];
+              if constexpr (ANY) { if (p.relu) ov = fmaxf(ov, 0.f); }
               yrow[cc] = ov;
               amax = fmaxf(amax, fabsf(ov));
             }
@@ -328,6 +386,40 @@ __global__ void __launch_bounds__(256) splitk_epilogue_kernel(const TcParams p, 
         if (p.rowadd) v += __ldg(p.rowadd + (long long)img * p.ld_rowadd + cc);
         if (p.residual) v += __ldg(p.residual + m * p.ld_res + cc);
         if (p.accumulate) v += yrow[cc];
+        yrow[cc] = v;
+        amax = fmaxf(amax, fabsf(v));
+      }
+    }
+  }
+  if (p.amax_out) amax_commit(p.amax_out, amax);
+}
+
+// The same for conv_tc_ps_kernel<true>: workspace row m is output pixel m of the flattened [M][ldy] view (rows past M are tile padding),
+// ReLU after the fixed-order sum of the splits.
+__global__ void __launch_bounds__(256) splitk_flat_epilogue_kernel(const TcParams p) {
+  const int c4 = (p.Nout + 3) >> 2;
+  const long long total = (long long)p.gM * c4;
+  float amax = 0.f;
+  for (long long i = blockIdx.x * 256ll + threadIdx.x; i < total; i += (long long)gridDim.x * 256) {
+    const long long m = i / c4;
+    const int c = (int)(i - m * c4) << 2;
+    const float* src = p.ws + m * p.ws_ld + c;
+    float4 acc = *reinterpret_cast<const float4*>(src);
+    for (int ks = 1; ks < p.ksplit; ++ks) {
+      const float4 t = *reinterpret_cast<const float4*>(src + ks * p.ws_split_stride);
+      acc.x += t.x; acc.y += t.y; acc.z += t.z; acc.w += t.w;
+    }
+    const float o[4] = {acc.x, acc.y, acc.z, acc.w};
+    float* yrow = p.y + m * p.ldy;
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const int cc = c + e;
+      if (cc < p.Nout) {
+        float v = o[e];
+        if (p.bias) v += __ldg(p.bias + cc);
+        if (p.residual) v += __ldg(p.residual + m * p.ld_res + cc);
+        if (p.accumulate) v += yrow[cc];
+        if (p.relu) v = fmaxf(v, 0.f);
         yrow[cc] = v;
         amax = fmaxf(amax, fabsf(v));
       }
@@ -563,7 +655,8 @@ int tc_init() {
   if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres) != cudaSuccess || !fn ||
       qres != cudaDriverEntryPointSuccess) { (void)cudaGetLastError(); return 0; }
   g_encode = (EncodeTiledFn)fn;
-  bool ok = cudaFuncSetAttribute(conv_tc_ps_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, PS_SMEM) == cudaSuccess;
+  bool ok = cudaFuncSetAttribute(conv_tc_ps_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, PS_SMEM) == cudaSuccess;
+  ok = ok && cudaFuncSetAttribute(conv_tc_ps_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, PS_SMEM) == cudaSuccess;
   ok = ok && cudaFuncSetAttribute(wgrad_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_SMEM) == cudaSuccess;
   cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev);
   if (!ok) { (void)cudaGetLastError(); return 0; }
@@ -684,7 +777,7 @@ int launch_tc(const float* act, long long ld_act, const uint32_t* amax_a, int Ni
     }
     const int work = total * p.ksplit;
     const int ctas = work < g_num_sms ? work : g_num_sms;
-    conv_tc_ps_kernel<<<ctas, THREADS, PS_SMEM, st>>>(mA, mBh, mBl, p, tiles_m, total);
+    conv_tc_ps_kernel<false><<<ctas, THREADS, PS_SMEM, st>>>(mA, mBh, mBl, p, tiles_m, total);
     if (p.ksplit > 1) {
       int rc = dp_check_launch();
       if (rc) return rc;
@@ -885,6 +978,7 @@ static TapTable dense_taps(int R, int S, int pad, bool flip) {
 
 int dp_conv2d_fprop_tc(const dp_conv_args* a, dp_stream_t stream) {
   if (!a || !a->x || !a->y) return DP_ERR_UNSUPPORTED;   // let the SIMT entry produce the precise error
+  if (a->flags & DP_CONV_RELU) return DP_ERR_UNSUPPORTED;  // the ReLU epilogue lives on the SIMT kernel
   if (a->R != a->S || (a->R != 1 && a->R != 3) || a->pad_l != a->pad_t) return DP_ERR_UNSUPPORTED;
   // stride 1: 'same' padding.  stride 2: 3x3 with pad 1, or pad 0 + the (0,1,0,1) zero border of Downsample2D (resnet.py:213-218) which
   // TMA out-of-bounds zero fill provides for free
@@ -895,6 +989,68 @@ int dp_conv2d_fprop_tc(const dp_conv_args* a, dp_stream_t stream) {
                    dense_taps(a->R, a->S, a->pad_t, false), 1, 0, 0, a->P, a->Q, (float*)a->y, a->ldy, a->bias, a->rowadd,
                    a->ld_rowadd, a->residual, a->ld_res, (a->flags & DP_CONV_ACCUMULATE) ? 1 : 0, (cudaStream_t)stream, 1.0f, 0, a->stride, -1,
                    a->workspace, nullptr, a->amax_out);
+}
+
+// General-geometry fprop (DP_CONV_ANY_GEOMETRY): any R x S, stride 1 or 2, explicit top / left padding, any N x H x W, on
+// conv_tc_ps_kernel<true>.  Channel counts below ANY_MIN_C stay on the SIMT kernel: a stage holds 64 input channels, and with fewer than 32
+// of them most of every 3 x fp16 product multiplies zero fill (Inception's C = 3 stem).  ws_need: geometry-only workspace query.
+constexpr int ANY_MIN_C = 32;
+int fprop_tc_any(const dp_conv_args* a, float* ws, long long* ws_need, cudaStream_t st) {
+  if (a->N <= 0 || a->H <= 0 || a->W <= 0 || a->C <= 0 || a->K <= 0 || a->P <= 0 || a->Q <= 0 || a->R <= 0 || a->S <= 0) return DP_ERR_UNSUPPORTED;
+  if (a->C < ANY_MIN_C || (a->stride != 1 && a->stride != 2) || a->pad_t < 0 || a->pad_l < 0 || a->rowadd) return DP_ERR_UNSUPPORTED;
+  if ((long long)a->N * a->P * a->Q >= (1ll << 31) || (long long)a->R * a->S > 65535) return DP_ERR_UNSUPPORTED;
+  if (!tc_init()) return DP_ERR_UNSUPPORTED;
+  const int M = a->N * a->P * a->Q, tiles_m = (M + BM - 1) / BM, n_tiles = (a->K + PS_BN - 1) / PS_BN;
+  const int kchunks = (a->C + BK - 1) / BK, iters = a->R * a->S * kchunks;
+  if (ws_need) {
+    int ips;
+    const int ks = pick_ksplit(tiles_m * n_tiles, iters, ips);
+    *ws_need = ks > 1 ? (long long)ks * tiles_m * BM * n_tiles * PS_BN : 0;
+    return DP_OK;
+  }
+  if (!a->x || !a->y || !a->w_tc_hi || !a->w_tc_lo || !a->amax_x || !a->amax_w) return DP_ERR_UNSUPPORTED;
+  if (a->ldx % 4 || ((uintptr_t)a->x & 15) || ((uintptr_t)a->w_tc_hi & 15) || ((uintptr_t)a->w_tc_lo & 15)) return DP_ERR_UNSUPPORTED;
+  CUtensorMap mBh, mBl;
+  {
+    const cuuint64_t Kp = (cuuint64_t)wrow(a->C);
+    cuuint64_t dims[3] = {Kp, (cuuint64_t)a->K, (cuuint64_t)(a->R * a->S)};
+    cuuint64_t str[2] = {Kp * 2, (cuuint64_t)a->K * Kp * 2};
+    cuuint32_t box[3] = {(cuuint32_t)BK, (cuuint32_t)PS_BN, 1};
+    if (!make_map(&mBh, a->w_tc_hi, 3, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B, 1, CU_TENSOR_MAP_DATA_TYPE_FLOAT16) ||
+        !make_map(&mBl, a->w_tc_lo, 3, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B, 1, CU_TENSOR_MAP_DATA_TYPE_FLOAT16)) return DP_ERR_UNSUPPORTED;
+  }
+  TcParams p{};
+  p.Nimg = 1; p.H = 1; p.W = M; p.Nout = a->K;
+  p.ntaps = a->R * a->S; p.kchunks = kchunks;
+  p.os = 1; p.oa = 0; p.ob = 0; p.Ho = 1; p.Wo = M;
+  p.alpha = 1.0f; p.b_from_img = 0; p.in_stride = 1; p.amax_a = a->amax_x; p.amax_b = a->amax_w; p.amax_out = a->amax_out;
+  p.bw = BM; p.bh = 1; p.bn = 1; p.tiles_w = tiles_m; p.tiles_h = 1;
+  p.y = (float*)a->y; p.ldy = a->ldy; p.bias = a->bias; p.residual = a->residual; p.ld_res = a->ld_res;
+  p.accumulate = (a->flags & DP_CONV_ACCUMULATE) ? 1 : 0;
+  auto al16 = [](const void* q, long long ld) { return q == nullptr || ((((uintptr_t)q) & 15) == 0 && (ld % 4) == 0); };
+  p.vec4 = (al16(a->y, a->ldy) && al16(a->bias, 0) && al16(a->residual, a->ld_res)) ? 1 : 0;
+  p.gx = (const float*)a->x; p.gldx = a->ldx; p.gH = a->H; p.gW = a->W; p.gC = a->C; p.gQ = a->Q; p.gPQ = a->P * a->Q; p.gS = a->S;
+  p.gstride = a->stride; p.gpad_t = a->pad_t; p.gpad_l = a->pad_l; p.gM = M; p.relu = (a->flags & DP_CONV_RELU) ? 1 : 0;
+  const int total = tiles_m * n_tiles;
+  p.ksplit = 1; p.it_per_split = iters;
+  if (ws) {
+    p.ksplit = pick_ksplit(total, iters, p.it_per_split);
+    p.ws = ws; p.ws_ld = n_tiles * PS_BN; p.ws_split_stride = (long long)tiles_m * BM * p.ws_ld;
+  }
+  const int work = total * p.ksplit;
+  conv_tc_ps_kernel<true><<<work < g_num_sms ? work : g_num_sms, THREADS, PS_SMEM, st>>>(mBh, mBh, mBl, p, tiles_m, total);
+  if (p.ksplit > 1) {
+    int rc = dp_check_launch();
+    if (rc) return rc;
+    long long blocks = ((long long)M * ((a->K + 3) / 4) + 255) / 256;
+    if (blocks > g_num_sms * 8) blocks = g_num_sms * 8;
+    splitk_flat_epilogue_kernel<<<(int)blocks, 256, 0, st>>>(p);
+  }
+  return dp_check_launch();
+}
+int dp_conv2d_fprop_tc_any(const dp_conv_args* a, dp_stream_t stream) {
+  if (!a) return DP_ERR_UNSUPPORTED;
+  return fprop_tc_any(a, a->workspace, nullptr, (cudaStream_t)stream);
 }
 
 // stride-1 dgrad == fprop of dy with the taps flipped and the (K,C) roles swapped: dx[n,h,w,c] = sum dy[n,h+1-r,w+1-s,k] W[k,c,r,s].
@@ -939,6 +1095,13 @@ int dp_conv2d_dgrad_tc(const dp_conv_args* a, dp_stream_t stream) {
 // Floats of split-K workspace dp_conv2d_fprop (op 0) / dp_conv2d_dgrad (op 1) can use for this geometry (0: the launch fills the SMs
 // without splitting).  With a->workspace == NULL the launch simply does not split.
 extern "C" long long dp_conv_splitk_workspace_floats(const dp_conv_args* a, int op) {
+  if (a && op == 0 && (a->flags & DP_CONV_ANY_GEOMETRY)) {   // the box kernel's need, or else the general-geometry kernel's
+    dp_conv_args b = *a;
+    b.flags &= ~DP_CONV_ANY_GEOMETRY;
+    long long need = (a->flags & DP_CONV_RELU) ? 0 : dp_conv_splitk_workspace_floats(&b, 0), any = 0;
+    if (fprop_tc_any(a, nullptr, &any, nullptr) == DP_OK && any > need) need = any;
+    return need;
+  }
   if (!a || a->N <= 0 || a->H <= 0 || a->W <= 0 || a->C <= 0 || a->K <= 0 || a->R != a->S || (a->R != 1 && a->R != 3)) return 0;
   long long need = 0;
   TapTable t{};

@@ -40,7 +40,8 @@ struct GemmParams {
   Gather g;
 };
 
-template <int AM, int BMODE>
+// RELU: y = max(y, 0) after every epilogue term (DP_CONV_RELU on fprop); a separate instantiation, so the others are unchanged
+template <int AM, int BMODE, bool RELU = false>
 __global__ void __launch_bounds__(NTHREADS) gemm_simt_kernel(const GemmParams p) {
   __shared__ __align__(16) float As[2][TK][TM + 4];
   __shared__ __align__(16) float Bs[2][TK][TN + 4];
@@ -243,6 +244,7 @@ __global__ void __launch_bounds__(NTHREADS) gemm_simt_kernel(const GemmParams p)
       if (radd) v += __ldg(radd + n);
       if (res) v += __ldg(res + n);
       if (p.accumulate) v += crow[n];
+      if (RELU) v = fmaxf(v, 0.f);
       crow[n] = v;
       amax = fmaxf(amax, fabsf(v));
     }
@@ -250,11 +252,11 @@ __global__ void __launch_bounds__(NTHREADS) gemm_simt_kernel(const GemmParams p)
   if (p.amax_out) amax_commit(p.amax_out, amax);
 }
 
-template <int AM, int BMODE>
+template <int AM, int BMODE, bool RELU = false>
 int launch_gemm(const GemmParams& p, int zdim, cudaStream_t st) {
   dim3 grid((p.M + TM - 1) / TM, (p.N + TN - 1) / TN, zdim);
   if (grid.y > 65535 || grid.z > 65535) return DP_ERR_SHAPE;
-  gemm_simt_kernel<AM, BMODE><<<grid, NTHREADS, 0, st>>>(p);
+  gemm_simt_kernel<AM, BMODE, RELU><<<grid, NTHREADS, 0, st>>>(p);
   return dp_check_launch();
 }
 
@@ -301,6 +303,7 @@ int dp_conv2d_fprop_simt(const dp_conv_args* a, dp_stream_t stream) {
   g.P = a->P; g.Q = a->Q; g.PQ = a->P * a->Q; g.S = a->S;
   g.sm = a->stride; g.sr = 1; g.off_h = -a->pad_t; g.off_w = -a->pad_l; g.sds = 0;
   g.logQ = ilog2_exact(g.Q); g.logPQ = ilog2_exact(g.PQ);
+  if (a->flags & DP_CONV_RELU) return launch_gemm<A_GATHER, B_NC, true>(p, 1, (cudaStream_t)stream);
   return launch_gemm<A_GATHER, B_NC>(p, 1, (cudaStream_t)stream);
 }
 

@@ -184,6 +184,8 @@ class DDIMPipeline:
                         image = self.scheduler.step(eps, t, image, eta=eta, generator=generator).prev_sample
         finally:
             self.unet.train(was_training)
+        if output_type == "device":   # the raw final sample, NCHW on the device (FID statistics quantise it there, fid.py)
+            return SimpleNamespace(images=image) if return_dict else (image,)
         image = (image / 2 + 0.5).clamp(0, 1).cpu().permute(0, 2, 3, 1).numpy()
         if output_type == "pil":
             from PIL import Image  # optional dependency, like the reference

@@ -53,6 +53,14 @@ int dp_tc_available(void);
  * ------------------------------------------------------------------------------------------------ */
 #define DP_CONV_ACCUMULATE 1 /* fprop: y += ; dgrad: dx += (instead of =) */
 #define DP_CONV_FORCE_SIMT 2 /* never take the tensor-core path (testing / odd shapes) */
+#define DP_CONV_RELU 4       /* fprop: y = max(y, 0) after bias / residual / accumulate (BasicConv2d of Inception-v3), after the fixed-order
+                                split-K sum; amax_out sees the rectified values.  The box tensor-core kernel declines it (general-geometry
+                                kernel or SIMT) */
+#define DP_CONV_ANY_GEOMETRY 8 /* fprop opt-in: when the box tensor-core kernel does not take the launch, run the general-geometry one
+                                (any R x S, stride 1 / 2, explicit top / left padding, any N x H x W; 128 flattened output pixels per tile,
+                                A gathered per tap with cp.async, same 3 x fp16 split, epilogue and split-K) before falling back to SIMT.
+                                Needs the same operands as the box kernel (w_tc_hi / lo, amax_x, amax_w, ldx % 4 == 0, 16-byte aligned x);
+                                input channel counts below 32 stay on SIMT, where they run faster.  rowadd is not supported there. */
 
 typedef struct dp_conv_args {
   int32_t N, H, W, C;
@@ -347,6 +355,31 @@ int dp_ddim_step(const float* x, const float* eps, const float* noise, float* ou
 
 /* y[i] = x[i] * s  (gradient averaging after all-reduce etc.) */
 int dp_scale(float* x, int64_t n, float s, dp_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * FID evaluation (fid.cu): the Inception-v3 feature pass of fid_score.py / inception.py around the convolutions.
+ * ------------------------------------------------------------------------------------------------ */
+/* Front end of InceptionV3.forward (inception.py:146-153) in one launch.  src: uint8 NHWC [N][Hs][Ws][3] (decoded RGB files, value
+ * (float)u / 255.0f as ToTensor computes it) when src_u8, else fp32 NCHW [N][3][Hs][Ws] in [0, 1]; with `quantize` (fp32 source only) each
+ * value is first taken through the sampler's PNG write, u = rint(clamp(x / 2 + 0.5, 0, 1) * 255) (round half to even, as numpy), which
+ * makes a DDIM sample in [-1, 1] read exactly like its saved PNG.  Then bilinear resize to Ho x Wo (align_corners = False, torch's
+ * source-index rule; resize = 0 requires Ho = Hs, Wo = Ws), then 2x - 1 when normalize.  out: NHWC [N][Ho][Wo] view, pixel stride
+ * ld_out >= 3.
+ * amax_out (optional): accumulates max|out| (dp_amax semantics), the slot the tensor-core convolution reading `out` needs. */
+int dp_fid_input(const void* src, int32_t src_u8, int32_t quantize, int32_t N, int32_t Hs, int32_t Ws, float* out, int64_t ld_out,
+                 int32_t Ho, int32_t Wo, int32_t resize, int32_t normalize, uint32_t* amax_out, dp_stream_t stream);
+/* 3 x 3 pooling over NHWC views, output extent P = (H + 2 pad - 3) / stride + 1 (floor, as torch):
+ *   mode 0: max (max_pool2d; padding never wins), mode 1: average with count_include_pad = False (FIDInceptionA / C / E_1),
+ *   the window sum taken row by row, left to right, then divided by the count of valid taps.  amax_out as in dp_fid_input. */
+int dp_pool3x3(const float* x, int64_t ldx, float* y, int64_t ldy, int32_t N, int32_t H, int32_t W, int32_t C, int32_t stride,
+               int32_t pad, int32_t mode, uint32_t* amax_out, dp_stream_t stream);
+/* y[n][c] = (sum_{h,w} x[n][h][w][c]) / H / W, summed in pixel order (adaptive_avg_pool2d to 1 x 1); y pitch ldy */
+int dp_global_mean(const float* x, int64_t ldx, float* y, int64_t ldy, int32_t N, int32_t H, int32_t W, int32_t C, dp_stream_t stream);
+/* Feature moments in fp64 over `rows` rows of an fp32 [rows][D] view, about a per-dimension shift d = f - shift (shift: fp32 [D], NULL =
+ * 0):  sum[i] += sum_r d[r][i],  sxx[i*D + j] += sum_r d[r][i] d[r][j] for j >= i (upper triangle; the lower one is not touched).  A shift
+ * near the mean (the first batch's) keeps the covariance from cancelling against mu mu^T.  Rows are summed in index order: results are
+ * run-to-run identical, and moments about the same shift from several batches (or devices) are plain sums. */
+int dp_feature_moments(const float* f, int64_t ld, int64_t rows, int32_t D, const float* shift, double* sum, double* sxx, dp_stream_t stream);
 
 #ifdef __cplusplus
 }

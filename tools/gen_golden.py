@@ -14,6 +14,7 @@ Outputs (all small, committed):
     tests/golden/cifar_cfg1_s3.pt  same with 3 timesteps (fast CPU check of the oracle)
     tests/golden/finetune_tiny.pt  2 finetune steps on TINY (Adam + clip + EMA), dropout 0
     tests/golden/ddim_tiny.pt      DDIMPipeline samples (uniform/eta 0/10 steps, quad/eta 0.5/7 steps) on TINY
+    tests/golden/fid_*             FID Inception fixtures (gen_fid): weight-file layout, features of seeded weights, Frechet cases
 """
 import argparse
 import hashlib
@@ -556,13 +557,85 @@ def gen_ref_pickle():
     print("ref_pickle", os.path.getsize(os.path.join(OUT, "ref_pruned_small.pth")), sum(p.numel() for p in m.parameters()))
 
 
+def gen_fid():
+    """FID fixtures from the UNMODIFIED inception.py / fid_score.py.  The weights are a seeded random state dict
+    (oracle.inception_oracle.seeded_state_dict): inception.py's module-level load_state_dict_from_url is replaced, before any
+    InceptionV3 is built, by a function returning it, so nothing is fetched.  Writes
+      fid_weights.json  the weight file's keys and shapes (torchvision names), the wrapper's keys, the seeded state dict's digest
+      fid_features.pt   uint8 input images (32x32, 64x64, 256x256) and their pool features for all four output blocks
+      fid_frechet.pt    (mu1, sigma1, mu2, sigma2) -> calculate_frechet_distance, including a product that takes the singular branch"""
+    import numpy as np
+    import torchvision.transforms as TF
+    from scipy import linalg
+    from oracle import inception_oracle as orc
+    import inception as ref_inception
+
+    tv = ref_inception._inception_v3(num_classes=1008, aux_logits=False, weights=None)
+    for name, block in (("Mixed_5b", ref_inception.FIDInceptionA(192, pool_features=32)),
+                        ("Mixed_5c", ref_inception.FIDInceptionA(256, pool_features=64)),
+                        ("Mixed_5d", ref_inception.FIDInceptionA(288, pool_features=64)),
+                        ("Mixed_6b", ref_inception.FIDInceptionC(768, channels_7x7=128)),
+                        ("Mixed_6c", ref_inception.FIDInceptionC(768, channels_7x7=160)),
+                        ("Mixed_6d", ref_inception.FIDInceptionC(768, channels_7x7=160)),
+                        ("Mixed_6e", ref_inception.FIDInceptionC(768, channels_7x7=192)),
+                        ("Mixed_7b", ref_inception.FIDInceptionE_1(1280)), ("Mixed_7c", ref_inception.FIDInceptionE_2(2048))):
+        setattr(tv, name, block)
+    shapes = [(k, list(v.shape)) for k, v in tv.state_dict().items()]
+    seeded = orc.seeded_state_dict(shapes, seed=0)
+
+    def offline_loader(url, *a, **kw):
+        assert url == ref_inception.FID_WEIGHTS_URL
+        return {k: v.clone() for k, v in seeded.items()}
+    ref_inception.load_state_dict_from_url = offline_loader
+    net = ref_inception.InceptionV3([0, 1, 2, 3]).eval()
+    json.dump({"weight_file": shapes, "wrapper": [(k, list(v.shape)) for k, v in net.state_dict().items()],
+               "seed": 0, "digest": orc.state_dict_digest(seeded)}, open(os.path.join(OUT, "fid_weights.json"), "w"))
+
+    g = torch.Generator().manual_seed(1)
+    images = {hw: torch.randint(0, 256, (2, hw, hw, 3), dtype=torch.uint8, generator=g) for hw in (32, 64, 256)}
+    feats = {}
+    with torch.no_grad():
+        for hw, u8 in images.items():
+            x = torch.stack([TF.ToTensor()(im.numpy()) for im in u8])      # fid_score.py:129 on HWC uint8, as PIL decoding yields
+            outs = net(x)
+            feats[hw] = [orc.pooled(o) for o in outs]
+            print("fid features", hw, [f"{float(f.abs().mean()):.3g}" for f in feats[hw]])
+    torch.save({"images": images, "features": feats}, os.path.join(OUT, "fid_features.pt"))
+
+    # fid_score.py calls sqrtm(..., disp=False), which scipy >= 1.16 no longer takes: give it that form back for the generator only
+    sqrtm = linalg.sqrtm
+
+    def sqrtm_disp(a, disp=True):
+        r = sqrtm(a)
+        return (r, 0.0) if not disp else r
+    linalg.sqrtm = sqrtm_disp
+    import fid_score as ref_fid
+    rng = np.random.default_rng(2)
+    cases = []
+    for n, d in ((50, 8), (40, 16)):
+        a, b = rng.standard_normal((n, d)), rng.standard_normal((n, d)) * 1.5 + 0.3
+        case = dict(mu1=a.mean(0), sigma1=np.cov(a, rowvar=False), mu2=b.mean(0), sigma2=np.cov(b, rowvar=False))
+        case["fid"] = float(ref_fid.calculate_frechet_distance(**case))
+        cases.append(case)
+    # sigma1 sigma2 = [[0, 1], [0, 0]] has no square root: the eps-offset retry runs, and its complex root fails the imaginary check
+    case = dict(mu1=np.zeros(2), sigma1=np.array([[0.0, 1.0], [1.0, 0.0]]), mu2=np.ones(2), sigma2=np.diag([0.0, 1.0]))
+    try:
+        case["fid"] = float(ref_fid.calculate_frechet_distance(**case))
+    except ValueError as e:
+        case["error"] = str(e)
+    cases.append(case)
+    linalg.sqrtm = sqrtm
+    torch.save(cases, os.path.join(OUT, "fid_frechet.pt"))
+    print("fid frechet", [c.get("fid", c.get("error")) for c in cases])
+
+
 if __name__ == "__main__":
     ap = argparse.ArgumentParser()
     ap.add_argument("--skip-cfg1", action="store_true")
     ap.add_argument("--only", default=None)
     a = ap.parse_args()
     torch.set_num_threads(os.cpu_count())
-    jobs = {"ldm_tiny": gen_ldm_tiny, "exp_importance": gen_exp_importance, "ref_pickle": gen_ref_pickle, "lsun_struct": gen_lsun_struct, "lr": gen_lr, "ckpt": gen_ckpt, "ddim": gen_ddim, "tiny": gen_tiny, "blocks": gen_blocks, "finetune": gen_finetune, "cifar_fwd": gen_cifar_fwd,
+    jobs = {"fid": gen_fid, "ldm_tiny": gen_ldm_tiny, "exp_importance": gen_exp_importance, "ref_pickle": gen_ref_pickle, "lsun_struct": gen_lsun_struct, "lr": gen_lr, "ckpt": gen_ckpt, "ddim": gen_ddim, "tiny": gen_tiny, "blocks": gen_blocks, "finetune": gen_finetune, "cifar_fwd": gen_cifar_fwd,
             "cfg1_s3": gen_cfg1_s3, "cfg3_s3": gen_cfg3_s3, "cfg1": gen_cfg1}
     for name, fn in jobs.items():
         if a.only and name != a.only:
