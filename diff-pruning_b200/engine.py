@@ -19,7 +19,6 @@ from __future__ import annotations
 
 import ctypes as C
 import math
-import os
 from typing import Callable, Dict, List, Optional, Tuple
 
 import torch
@@ -36,13 +35,13 @@ _SM_COUNT = 132            # H100 SXM; the wgrad kernel runs one CTA per SM (192
 _WGRAD_CTA_OVERHEAD = 8    # per-CTA prologue + pipeline fill + register->workspace epilogue, in units of one 64-pixel stage
 
 
-def _wgrad_splits(tiles, chunks, env=os.environ.get("DPB200_WGRAD_WAVES")):
+def _wgrad_splits(tiles, chunks):
     """Split-K factor of the tensor-core wgrad: grid = tiles x splits CTAs, each walking ceil(chunks / splits) pixel chunks.
     One CTA per SM, so the launch runs in ceil(grid / 132) strict waves: pick the split count whose modelled time
     waves x (overhead + chunks per CTA) is smallest (ties: fewer splits = smaller workspace), so a grid never overshoots a
-    wave boundary by a few CTAs (530 CTAs would cost a fifth, almost empty, wave) and no trailing split is empty."""
-    max_waves = int(env) if env else 8
-    hi = max(1, min(chunks, max(2, (max_waves * _SM_COUNT) // tiles)))
+    wave boundary by a few CTAs (530 CTAs would cost a fifth, almost empty, wave) and no trailing split is empty.
+    The search stops at 8 waves' worth of CTAs."""
+    hi = max(1, min(chunks, max(2, (8 * _SM_COUNT) // tiles)))
     best = None
     for sp in range(1, hi + 1):
         cps = -(-chunks // sp)
@@ -56,6 +55,11 @@ def _wgrad_splits(tiles, chunks, env=os.environ.get("DPB200_WGRAD_WAVES")):
 
 def _stream() -> int:
     return torch.cuda.current_stream().cuda_stream
+
+
+def _wgeom(w: torch.Tensor) -> Tuple[int, int, int, int]:
+    """(K, Cin, R, S) of an OIHW convolution weight or an (out, in) linear weight (a 1x1 convolution)."""
+    return (w.shape[0], w.shape[1], w.shape[2], w.shape[3]) if w.dim() == 4 else (w.shape[0], w.shape[1], 1, 1)
 
 
 class View:
@@ -98,12 +102,44 @@ def _copy_args(a):
     return b
 
 
+def _epilogue(a, b, rowadd, residual, accumulate_out):
+    """The fprop epilogue of a ConvArgs / ConvBf16Args: out (= or +=) conv + bias + per-image row + residual."""
+    a.flags = 1 if accumulate_out else 0
+    a.bias = b.data_ptr() if b is not None else None
+    if rowadd is not None:
+        a.rowadd, a.ld_rowadd = rowadd.ptr, rowadd.ld
+    if residual is not None:
+        a.residual, a.ld_res = residual.ptr, residual.ld
+
+
+def _bwd_args(a):
+    """A convolution's wgrad / dgrad argument struct: its fprop struct without the fprop epilogue."""
+    b = _copy_args(a)
+    b.flags = 0
+    b.rowadd = b.residual = b.bias = b.workspace = None
+    return b
+
+
+def _to_side(steps: List[Step], first: int):
+    """steps[first:] run as one group on the side stream; the group's first launch waits for the main stream's progress so far."""
+    for f in steps[first:]:
+        f.side = 1
+    steps[first].side = 2
+
+
+def h_half(skip: View) -> View:
+    """Channels [0, C_h) of a skip's concat buffer: the h half of torch.cat([h, skip]), written by the up path."""
+    return View(skip.t, 0, skip.off)
+
+
+def cat_of(skip: View) -> View:
+    """The whole torch.cat([h, skip]) buffer a skip view lives in."""
+    return View(skip.t, 0, skip.off + skip.C)
+
+
 AMAX_SLOTS = 8192  # capacity of a plan's amax-slot arrays (one uint32 per tensor-core operand use)
 AUDIT_SLOTS = False  # tests: plans built while this is set check every amax slot against torch.amax of its operand right before the
                      # consuming launch (eager runs only: the check synchronises)
-SIDE_WGRAD = True  # backward: weight-gradient launches (wgrad + split-K reduce) run on a second stream.  They only feed Parameter.grad, so the
-                   # dgrad -> GroupNorm chain does not wait for them, and the small latency-bound kernels of that chain share SMs with wgrad CTAs
-SPLITK = True      # small-M fprop / dgrad launches split their K loop over idle SMs (dp_conv_splitk_workspace_floats)
 ARENA_ALIGN = 64   # floats: every parameter's slice of a flat arena starts on a 256-byte boundary
 
 
@@ -292,9 +328,7 @@ class Plan:
         got = self._packs.get(id(w))
         if got is not None:
             return got
-        K, Cin = w.shape[0], w.shape[1]
-        R = w.shape[2] if w.dim() == 4 else 1
-        S = w.shape[3] if w.dim() == 4 else 1
+        K, Cin, R, S = _wgeom(w)
         wck = torch.empty(w.numel(), device=self.dev, dtype=torch.float32)
         wkc = torch.empty(w.numel(), device=self.dev, dtype=torch.float32)
         lib = self.lib
@@ -401,9 +435,8 @@ class Plan:
     def _bf_geom(self, x: View, out: View, w: nn.Parameter, stride: int, pad: int) -> "L.ConvBf16Args":
         a = L.ConvBf16Args()
         a.N, a.H, a.W, a.C = x.N, x.H, x.W, x.C
-        a.P, a.Q, a.K = out.H, out.W, w.shape[0]
-        a.R = w.shape[2] if w.dim() == 4 else 1
-        a.S = w.shape[3] if w.dim() == 4 else 1
+        a.P, a.Q = out.H, out.W
+        a.K, _, a.R, a.S = _wgeom(w)
         a.stride, a.pad_t, a.pad_l, a.splits = stride, pad, pad, 1
         a.ldx, a.lddy, a.ld_out = (x.C + 7) // 8 * 8, (w.shape[0] + 7) // 8 * 8, max(out.ld, x.ld)
         return a
@@ -440,9 +473,7 @@ class Plan:
     def _packed_bf16(self, w: nn.Parameter):
         got = self._bf_packs.get(id(w))
         if got is None:
-            K, Cin = w.shape[0], w.shape[1]
-            R = w.shape[2] if w.dim() == 4 else 1
-            S = w.shape[3] if w.dim() == 4 else 1
+            K, Cin, R, S = _wgeom(w)
             lib = self.lib
             kc = torch.empty(R * S * K * lib.dp_bf16_weight_row(Cin), device=self.dev, dtype=torch.bfloat16)
             ck = torch.empty(R * S * Cin * lib.dp_bf16_weight_row(K), device=self.dev, dtype=torch.bfloat16)
@@ -473,21 +504,94 @@ class Plan:
             if last:
                 return out_name
 
+    def _bias_grad(self, steps: List[Step], b: Optional[nn.Parameter], out: View, seg_out: Optional[str], dy_dense: Optional[str],
+                   side: bool):
+        """Per-image column sums of dy (left in the scratch `seg_out` when the caller reads them) and, with a bias, their sum over the
+        images into b.grad.  A dense dy (`dy_dense`, one row per image) is its own per-image sums.  side: the launches run as one
+        side-stream group, with column-sum scratch of their own."""
+        lib, K, n0 = self.lib, out.C, len(steps)
+        if dy_dense is not None:
+            seg = dy_dense
+        else:
+            dout = self.gradof(out)
+            seg = self._colsum_tree(steps, dout.ptr, dout.ld, out.rows, out.H * out.W, K, seg_out,
+                                    ("cs_a_side", "cs_b_side") if side else ("cs_a", "cs_b"))
+        if b is not None:
+            self._rec(steps, lambda s: lib.dp_colsum(self.sptr(seg), K, out.N, K, out.N, self.pgrad(b), K, 1, s), what="bias grad")
+        if side:
+            _to_side(steps, n0)
+
+    def _wgrad(self, steps: List[Step], fn, wa, w: nn.Parameter, b: Optional[nn.Parameter], rows: int, ctile: int, side: bool,
+               scores: bool, info: str):
+        """Weight gradient of one convolution: fn(wa) writes split-K partials of dW (and of db when `b` is given: the bias gradient
+        falls out of the same pass over dy) into a workspace, then dp_conv2d_wgrad_reduce sums them in a fixed order into w.grad
+        (b.grad), and into the signed Taylor scores of w when `scores`.  The caller binds wa's dy operand; ctile is the kernel's
+        in-channel tile width.
+        side: both launches run on the side stream, with workspaces of their own.  A weight gradient only feeds Parameter.grad, so the
+        dgrad -> GroupNorm chain does not wait for it, and the small latency-bound kernels of that chain share the SMs with its CTAs."""
+        K, Cin, R, S = _wgeom(w)
+        tiles = ((K + 127) // 128) * ((Cin + ctile - 1) // ctile) * R * S   # the kernel's grid: out-channel x in-channel tiles x taps
+        splits = _wgrad_splits(tiles, max(1, rows // 64))                   # the kernel walks 64-pixel chunks
+        ws, bws = ("wgrad_ws_side", "bias_ws_side") if side else ("wgrad_ws", "bias_ws")
+        self.scratch(ws, splits * K * R * S * Cin)
+        wa.splits = splits
+        ra = L.WgradReduceArgs()
+        ra.K, ra.C, ra.R, ra.S, ra.splits = K, Cin, R, S, splits
+        ra.dw = self.pgrad(w)
+        if scores:   # signed first-order Taylor terms sum_k W*dW_t fall out of the split-K reduce (ddpm_prune.py:60)
+            so, si = self._score_views(w, K, Cin)
+            ra.w, ra.score_out, ra.score_in = w.data_ptr(), so.data_ptr(), si.data_ptr()
+        if b is not None:
+            self.scratch(bws, splits * K)
+            ra.db = self.pgrad(b)
+
+        def bind():
+            for a in (wa, ra):
+                a.workspace = self.sptr(ws)
+                if b is not None:
+                    a.bias_ws = self.sptr(bws)
+        self._late.append(bind)
+        self._rec(steps, fn, wa, "conv wgrad", info)
+        self._rec(steps, self.lib.dp_conv2d_wgrad_reduce, ra, "conv wgrad reduce")
+        if side:
+            _to_side(steps, len(steps) - 2)
+
+    def _dgrad_target(self, it: BItem, da, x: View, dx_scratch: Optional[str], dx_into: Optional[View], field: str = "x",
+                      ld_field: str = "ldx", amax: bool = True):
+        """Points the dgrad struct's output (`field` / `ld_field`) at the shared dense scratch `dx_scratch` ([rows][C]), or at the
+        gradient view of `dx_into` / `x`: there the launch stores (=) when it is that gradient's first writer in execution order and
+        accumulates (+=) otherwise.  amax: the launch reports max|dx| to the gradient's consumers."""
+        if dx_scratch is not None:
+            self.scratch(dx_scratch, x.rows * x.C)
+            setattr(da, ld_field, x.C)
+            self._late.append(lambda: setattr(da, field, self.sptr(dx_scratch)))
+            return
+        tgt = dx_into if dx_into is not None else x
+        gx = self.gradof(tgt)
+        setattr(da, field, gx.ptr)
+        setattr(da, ld_field, gx.ld)
+        it.writes.append((tgt, lambda init: setattr(da, "flags", 1 if init else 0),
+                          (lambda slot: setattr(da, "amax_out", slot)) if amax else None))
+
     def conv(self, x: View, w: nn.Parameter, b: Optional[nn.Parameter], out: View, stride=1, pad=1,
              rowadd: Optional[View] = None, residual: Optional[View] = None, accumulate_out=False, need_dx=True,
              dx_scratch: Optional[str] = None, seg_out: Optional[str] = None, dy_dense: Optional[str] = None,
              dx_into: Optional[View] = None):
         """Records fprop (fwd) and bias-grad / wgrad / dgrad (bwd).
         dgrad target: `dx_scratch` (shared dense scratch [rows][C]) or the gradient view of `dx_into` / `x`.
-        dy source: out.grad, or the dense scratch `dy_dense` ([rows][K]) when the consumer provides it."""
+        dy source: out.grad, or the dense scratch `dy_dense` ([rows][K], one row per image) when the consumer provides it."""
         lib = self.lib
-        K, Cin = w.shape[0], w.shape[1]
-        R = w.shape[2] if w.dim() == 4 else 1
-        S = w.shape[3] if w.dim() == 4 else 1
+        K, Cin, R, S = _wgeom(w)
         assert x.C == Cin and out.C == K, (x.C, Cin, out.C, K)
-        use_bf = dy_dense is None and self.conv_bf16_ok(x, out, w, stride, pad, need_dx)
-        if use_bf:
-            return self._conv_bf16(x, w, b, out, stride, pad, rowadd, residual, accumulate_out, need_dx, dx_scratch, seg_out, dx_into)
+        assert dy_dense is None or out.H * out.W == 1, "a dense dy holds one row per image"
+        info = f"{Cin}->{K} {R}x{S}" + (f" s{stride}" if stride != 1 else "") + f" @{out.H}x{out.W}"
+        if w.dim() == 4:
+            self.conv_macs += out.rows * K * Cin * R * S      # 4-D-weight convolutions only: the roofline denominator (SURVEY.md §8d)
+        else:
+            self.lin_macs += out.rows * K * Cin               # nn.Linear layers (the LDM transformer blocks are linear-heavy)
+        if dy_dense is None and self.conv_bf16_ok(x, out, w, stride, pad, need_dx):
+            return self._conv_bf16(x, w, b, out, stride, pad, rowadd, residual, accumulate_out, need_dx, dx_scratch, seg_out, dx_into,
+                                   info + " bf16")
         wck, wkc, wtc = self._packed(w)
         a = L.ConvArgs()
         if wtc is not None:
@@ -496,21 +600,11 @@ class Plan:
         a.N, a.H, a.W, a.C = x.N, x.H, x.W, x.C
         a.P, a.Q, a.K = out.H, out.W, K
         a.R, a.S, a.stride, a.pad_t, a.pad_l = R, S, stride, pad, pad
-        a.flags = 1 if accumulate_out else 0
         a.splits = 1
         a.x, a.ldx, a.y, a.ldy = x.ptr, x.ld, out.ptr, out.ld
         a.amax_out = self._out_slot(out)
         a.w = wck.data_ptr()
-        a.bias = b.data_ptr() if b is not None else None
-        if rowadd is not None:
-            a.rowadd, a.ld_rowadd = rowadd.ptr, rowadd.ld
-        if residual is not None:
-            a.residual, a.ld_res = residual.ptr, residual.ld
-        info = f"{Cin}->{K} {R}x{S}" + (f" s{stride}" if stride != 1 else "") + f" @{out.H}x{out.W}"
-        if w.dim() == 4:
-            self.conv_macs += out.rows * K * Cin * R * S      # 4-D-weight convolutions only: the roofline denominator (SURVEY.md §8d)
-        else:
-            self.lin_macs += out.rows * K * Cin               # nn.Linear layers (the LDM transformer blocks are linear-heavy)
+        _epilogue(a, b, rowadd, residual, accumulate_out)
         self._splitk(a, 0)
         self._rec(self.fwd, lib.dp_conv2d_fprop, a, "conv fprop", info)
         if not self.need_grad:
@@ -518,101 +612,44 @@ class Plan:
         it = self._bitem()
         steps = it.steps
         # The time-embedding branch of a resnet (per-image sums of conv1's dy -> bias / time_emb_proj gradients -> d silu(temb)) only meets
-        # the main chain again at the very end of the backward: all of it runs on the side stream (fp32-grade plans; scratch of its own)
-        temb_side = SIDE_WGRAD and not self.bf16 and (dy_dense is not None or seg_out is not None)
-        n_steps0 = len(steps)
+        # the main chain again at the very end of the backward: all of it runs on the side stream, with scratch of its own.  Not in bf16
+        # plans: there a bf16 conv1 takes its per-image sums on the main stream.
+        temb_side = not self.bf16 and (dy_dense is not None or seg_out is not None)
         if dy_dense is not None:
             self.scratch(dy_dense, out.rows * K)
-            dy_get, dy_ld = (lambda n=dy_dense: self.sptr(n)), K
+            dy_get, dy_ld = (lambda: self.sptr(dy_dense)), K
         else:
             dout = self.gradof(out)
-            dy_get, dy_ld = (lambda p=dout.ptr: p), dout.ld
+            dy_get, dy_ld = (lambda: dout.ptr), dout.ld
         # 1. bias gradient (and per-image sums for the caller when seg_out is set).  Without seg_out the bias gradient falls out of the
         #    wgrad kernel's pass over dy (bias_ws -> dp_conv2d_wgrad_reduce): no column-sum launches at all
         bias_in_wgrad = b is not None and seg_out is None and dy_dense is None
         if (b is not None or seg_out is not None) and not bias_in_wgrad:
-            if dy_dense is not None and out.H * out.W == 1:
-                seg = dy_dense  # already dense per-image rows
-            else:
-                seg = None
-            if seg is None:
-                # src pointer may be late-bound (dense scratch) -> wrap
-                if dy_dense is not None:
-                    raise NotImplementedError("dense dy with spatial extent")
-                seg = self._colsum_tree(steps, dout.ptr, dout.ld, out.rows, out.H * out.W, K, seg_out,
-                                        ("cs_a_side", "cs_b_side") if temb_side else ("cs_a", "cs_b"))
-            if b is not None:
-                self._rec(steps, lambda s, seg=seg, b=b, n=x.N: lib.dp_colsum(self.sptr(seg), K, n, K, n, self.pgrad(b), K, 1, s),
-                          what="bias grad")
-            if temb_side:
-                for f in steps[n_steps0:]:
-                    f.side = 1
-                steps[n_steps0].side = 2
-        # 2. wgrad -> split-K workspace -> fixed-order reduce into Parameter.grad
-        TC = R * S * Cin
-        tiles = ((K + 127) // 128) * ((Cin + 127) // 128) * R * S   # the kernel's grid: out-channel tiles x in-channel tiles x taps
-        chunks = max(1, out.rows // 64)              # tensor-core wgrad walks 64-pixel chunks
-        splits = _wgrad_splits(tiles, chunks)
-        # dy in a per-tensor gradient buffer stays valid for the rest of the backward: its weight gradient may run on the side stream
-        # (own scratch: the main stream's wgrads — the temb projections, whose dy lives in a reused scratch — must not share it)
-        side = SIDE_WGRAD and (dy_dense is None or temb_side)
-        ws_name, bws_name = ("wgrad_ws_side", "bias_ws_side") if side else ("wgrad_ws", "bias_ws")
+            self._bias_grad(steps, b, out, seg_out, dy_dense, temb_side)
+        # 2. wgrad.  dy in a per-tensor gradient buffer stays valid for the rest of the backward, so its weight gradient may run on the
+        #    side stream; a dense dy lives in a reused scratch, so its weight gradient stays on the main stream outside the
+        #    time-embedding branch
         n_steps1 = len(steps)
-        self.scratch(ws_name, splits * K * TC)
         amax_dy = None
         if wtc is not None:
             amax_dy = self._amax(steps, dy_get, dy_ld, out.rows, K) if dy_dense is not None else self._dy_slot(steps, out)
-        wa = _copy_args(a)
-        wa.amax_y, wa.amax_out = amax_dy, None
-        wa.flags, wa.splits = 0, splits
-        wa.ldy = dy_ld
-        wa.rowadd, wa.residual, wa.bias = None, None, None
-        self._late.append(lambda wa=wa, g=dy_get, n=ws_name: (setattr(wa, "y", g()), setattr(wa, "workspace", self.sptr(n))))
-        if bias_in_wgrad:
-            self.scratch(bws_name, splits * K)
-            self._late.append(lambda wa=wa, n=bws_name: setattr(wa, "bias_ws", self.sptr(n)))
-        self._rec(steps, lib.dp_conv2d_wgrad, wa, "conv wgrad", info)
-        steps[-1].side = 2 if side else 0          # 2: first launch of a side group (waits for the main stream's progress so far)
-        ra = L.WgradReduceArgs()
-        ra.K, ra.C, ra.R, ra.S, ra.splits = K, Cin, R, S, splits
-        ra.dw = self.pgrad(w)
-        if self.fused_scores:   # signed first-order Taylor terms sum_k W*dW_t fall out of the split-K reduce (ddpm_prune.py:60)
-            so, si = self._score_views(w, K, Cin)
-            ra.w, ra.score_out, ra.score_in = w.data_ptr(), so.data_ptr(), si.data_ptr()
-        self._late.append(lambda ra=ra, n=ws_name: setattr(ra, "workspace", self.sptr(n)))
-        if bias_in_wgrad:
-            ra.db = self.pgrad(b)
-            self._late.append(lambda ra=ra, n=bws_name: setattr(ra, "bias_ws", self.sptr(n)))
-        self._rec(steps, lib.dp_conv2d_wgrad_reduce, ra, "conv wgrad reduce")
-        steps[-1].side = 1 if side else 0
+        wa = _bwd_args(a)
+        wa.ldy, wa.amax_y, wa.amax_out = dy_ld, amax_dy, None
+        self._late.append(lambda: setattr(wa, "y", dy_get()))
+        self._wgrad(steps, lib.dp_conv2d_wgrad, wa, w, b if bias_in_wgrad else None, out.rows, 128,
+                    side=dy_dense is None or temb_side, scores=self.fused_scores, info=info)
         # 3. dgrad
         if need_dx:
-            da = _copy_args(a)
-            da.ldy = dy_ld
-            da.w = wkc.data_ptr()
+            da = _bwd_args(a)
+            da.w, da.ldy, da.amax_out = wkc.data_ptr(), dy_ld, None
             if wtc is not None:
                 da.w_tc_hi, da.w_tc_lo, da.amax_y = wtc[2].data_ptr(), wtc[3].data_ptr(), amax_dy
-            da.flags = 0
-            da.amax_out = None
-            da.rowadd, da.residual, da.bias = None, None, None
-            self._late.append(lambda da=da, g=dy_get: setattr(da, "y", g()))
-            if dx_scratch is not None:
-                self.scratch(dx_scratch, x.rows * x.C)
-                da.ldx = x.C
-                self._late.append(lambda da=da, n=dx_scratch: setattr(da, "x", self.sptr(n)))
-            else:
-                tgt = dx_into if dx_into is not None else x
-                gx = self.gradof(tgt)
-                da.x, da.ldx = gx.ptr, gx.ld
-                it.writes.append((tgt, lambda init, da=da: setattr(da, "flags", 1 if init else 0),
-                                  lambda slot, da=da: setattr(da, "amax_out", slot)))
-            da.workspace = None
+            self._late.append(lambda: setattr(da, "y", dy_get()))
+            self._dgrad_target(it, da, x, dx_scratch, dx_into)
             self._splitk(da, 1, "splitk_ws_side" if (temb_side and dy_dense is not None) else "splitk_ws")
             self._rec(steps, lib.dp_conv2d_dgrad, da, "conv dgrad", info)
         if temb_side and dy_dense is not None:      # the time_emb_proj convolution: amax(dy), wgrad, reduce, dgrad all on the side stream
-            for f in steps[n_steps1:]:
-                f.side = 1
-            steps[n_steps1].side = 2
+            _to_side(steps, n_steps1)
 
     FUSE_QKV = True      # to_q / to_k / to_v of an attention block as one projection (conv_qkv); tests / A-B runs may clear it before planning
 
@@ -679,88 +716,41 @@ class Plan:
         if ip != inner:
             dout.t.zero_()                 # pad columns of dy: read by the fused dgrad (against zero weights), written by nobody
         amax_dy = self._dy_slot(steps, qkv)
-        # weight (and bias) gradients: one launch per Parameter over its channel range of dy, side stream
+        # weight (and bias) gradients: one launch per Parameter over its channel range of dy (a gradient buffer of its own: side stream)
         pinfo = f"{Cin}->{inner} 1x1 @{x.H}x{x.W}"
-        tiles = ((inner + 127) // 128) * ((Cin + 127) // 128)
-        splits = _wgrad_splits(tiles, max(1, qkv.rows // 64))
-        side = SIDE_WGRAD
-        ws_name, bws_name = ("wgrad_ws_side", "bias_ws_side") if side else ("wgrad_ws", "bias_ws")
-        self.scratch(ws_name, splits * inner * Cin)
-        if has_bias:
-            self.scratch(bws_name, splits * inner)
         for i, (w, b) in enumerate(zip(ws, bs)):
-            wa = _copy_args(a)
-            wa.K = inner
-            wa.y, wa.ldy = dout.ptr + 4 * i * ip, dout.ld
-            wa.amax_y, wa.amax_out = amax_dy, None
-            wa.flags, wa.splits = 0, splits
-            wa.rowadd, wa.residual, wa.bias, wa.workspace = None, None, None, None
-            self._late.append(lambda wa=wa, n=ws_name: setattr(wa, "workspace", self.sptr(n)))
-            if has_bias:
-                self._late.append(lambda wa=wa, n=bws_name: setattr(wa, "bias_ws", self.sptr(n)))
-            self._rec(steps, lib.dp_conv2d_wgrad, wa, "conv wgrad", pinfo)
-            steps[-1].side = 2 if side else 0
-            ra = L.WgradReduceArgs()
-            ra.K, ra.C, ra.R, ra.S, ra.splits = inner, Cin, 1, 1, splits
-            ra.dw = self.pgrad(w)
-            if self.fused_scores:
-                so, si = self._score_views(w, inner, Cin)
-                ra.w, ra.score_out, ra.score_in = w.data_ptr(), so.data_ptr(), si.data_ptr()
-            self._late.append(lambda ra=ra, n=ws_name: setattr(ra, "workspace", self.sptr(n)))
-            if has_bias:
-                ra.db = self.pgrad(b)
-                self._late.append(lambda ra=ra, n=bws_name: setattr(ra, "bias_ws", self.sptr(n)))
-            self._rec(steps, lib.dp_conv2d_wgrad_reduce, ra, "conv wgrad reduce")
-            steps[-1].side = 1 if side else 0
+            wa = _bwd_args(a)
+            wa.K, wa.y, wa.ldy, wa.amax_y, wa.amax_out = inner, dout.ptr + 4 * i * ip, dout.ld, amax_dy, None
+            self._wgrad(steps, lib.dp_conv2d_wgrad, wa, w, b, qkv.rows, 128, side=True, scores=self.fused_scores, info=pinfo)
         # one dgrad over all 3 inner channels of dy
-        da = _copy_args(a)
-        da.y, da.ldy = dout.ptr, dout.ld
-        da.w = wkc.data_ptr()
+        da = _bwd_args(a)
+        da.y, da.ldy, da.w, da.amax_out = dout.ptr, dout.ld, wkc.data_ptr(), None
         da.w_tc_hi, da.w_tc_lo, da.amax_y = wtc[2].data_ptr(), wtc[3].data_ptr(), amax_dy
-        da.flags = 0
-        da.amax_out = None
-        da.rowadd, da.residual, da.bias = None, None, None
-        gx = self.gradof(x)
-        da.x, da.ldx = gx.ptr, gx.ld
-        it.writes.append((x, lambda init, da=da: setattr(da, "flags", 1 if init else 0),
-                          lambda slot, da=da: setattr(da, "amax_out", slot)))
-        da.workspace = None
+        self._dgrad_target(it, da, x, None, None)
         self._splitk(da, 1)
         self._rec(steps, lib.dp_conv2d_dgrad, da, "conv dgrad", info)
         return parts
 
     def _splitk(self, a, op: int, name: str = "splitk_ws"):
         """Small-M launches (4x4 .. 16x16 levels) split their K loop over the idle SMs: one shared scratch, bound late."""
-        need = int(self.lib.dp_conv_splitk_workspace_floats(C.byref(a), op)) if SPLITK else 0
+        need = int(self.lib.dp_conv_splitk_workspace_floats(C.byref(a), op))
         if need > 0:
             self.scratch(name, need)
             self._late.append(lambda a=a, n=name: setattr(a, "workspace", self.sptr(n)))
 
-    def _conv_bf16(self, x, w, b, out, stride, pad, rowadd, residual, accumulate_out, need_dx, dx_scratch, seg_out, dx_into):
+    def _conv_bf16(self, x, w, b, out, stride, pad, rowadd, residual, accumulate_out, need_dx, dx_scratch, seg_out, dx_into, info):
         """conv() on the bf16 tensor tier: same launch structure and fp32 outputs, operands as bf16 copies."""
         lib = self.lib
-        K, Cin = w.shape[0], w.shape[1]
-        R = w.shape[2] if w.dim() == 4 else 1
-        S = w.shape[3] if w.dim() == 4 else 1
+        K, Cin, _, _ = _wgeom(w)
         kc, ck = self._packed_bf16(w)
         xb, ldxb = self._bf16_of(x)
         self.n_bf16_convs += 1
         self._unslotted(out)        # the bf16 kernels do not report max|out|
         a = self._bf_geom(x, out, w, stride, pad)
-        a.flags = 1 if accumulate_out else 0
         a.x_bf16, a.ldx = xb.data_ptr(), ldxb
         a.out, a.ld_out = out.ptr, out.ld
         a.w_bf16 = kc.data_ptr()
-        a.bias = b.data_ptr() if b is not None else None
-        if rowadd is not None:
-            a.rowadd, a.ld_rowadd = rowadd.ptr, rowadd.ld
-        if residual is not None:
-            a.residual, a.ld_res = residual.ptr, residual.ld
-        info = f"{Cin}->{K} {R}x{S}" + (f" s{stride}" if stride != 1 else "") + f" @{out.H}x{out.W} bf16"
-        if w.dim() == 4:
-            self.conv_macs += out.rows * K * Cin * R * S
-        else:
-            self.lin_macs += out.rows * K * Cin
+        _epilogue(a, b, rowadd, residual, accumulate_out)
         self._rec(self.fwd, lib.dp_conv2d_fprop_bf16, a, "conv fprop", info)
         if not self.need_grad:
             return
@@ -769,47 +759,25 @@ class Plan:
         dout = self.gradof(out)
         # 1. bias gradient / per-image sums (fp32, from the fp32 dy)
         if b is not None or seg_out is not None:
-            seg = self._colsum_tree(steps, dout.ptr, dout.ld, out.rows, out.H * out.W, K, seg_out)
-            if b is not None:
-                self._rec(steps, lambda s, seg=seg, b=b, n=x.N: lib.dp_colsum(self.sptr(seg), K, n, K, n, self.pgrad(b), K, 1, s),
-                          what="bias grad")
+            self._bias_grad(steps, b, out, seg_out, None, side=False)
         # 2. dy -> bf16 once for wgrad and dgrad
         lddyb = (K + 7) // 8 * 8
         self.scratch("dy_bf16", (out.rows * lddyb + 1) // 2)
         self._rec(steps, lambda s, p=dout.ptr, ld=dout.ld, r=out.rows: lib.dp_cvt_bf16(p, ld, r, K, self.sptr("dy_bf16"), lddyb, s),
                   what="cvt bf16")
-        # 3. wgrad -> split-K workspace -> fixed-order reduce into Parameter.grad
-        TC = R * S * Cin
-        ctw = lib.dp_bf16_wgrad_ctile(Cin)
-        tiles = ((K + 127) // 128) * ((Cin + ctw - 1) // ctw) * R * S
-        chunks = max(1, out.rows // 64)
-        splits = _wgrad_splits(tiles, chunks)
-        self.scratch("wgrad_ws", splits * K * TC)
-        wa = _copy_args(a)
-        wa.flags, wa.splits, wa.lddy = 0, splits, lddyb
-        wa.rowadd, wa.residual, wa.bias, wa.out = None, None, None, None
-        self._late.append(lambda wa=wa: (setattr(wa, "dy_bf16", self.sptr("dy_bf16")), setattr(wa, "workspace", self.sptr("wgrad_ws"))))
-        self._rec(steps, lib.dp_conv2d_wgrad_bf16, wa, "conv wgrad", info)
-        ra = L.WgradReduceArgs()
-        ra.K, ra.C, ra.R, ra.S, ra.splits = K, Cin, R, S, splits
-        ra.dw = self.pgrad(w)
-        self._late.append(lambda ra=ra: setattr(ra, "workspace", self.sptr("wgrad_ws")))
-        self._rec(steps, lib.dp_conv2d_wgrad_reduce, ra, "conv wgrad reduce")
-        # 4. dgrad
+        # 3. wgrad, 4. dgrad.  Both stay on the main stream: their dy operand is the one shared dy_bf16 scratch, which the next
+        #    convolution's cvt bf16 overwrites
+        wa = _bwd_args(a)
+        wa.lddy, wa.out = lddyb, None
+        self._late.append(lambda: setattr(wa, "dy_bf16", self.sptr("dy_bf16")))
+        # no fused scores: their one user, TaylorScorer, plans fp32
+        self._wgrad(steps, lib.dp_conv2d_wgrad_bf16, wa, w, None, out.rows, lib.dp_bf16_wgrad_ctile(Cin), side=False, scores=False,
+                    info=info)
         if need_dx:
-            da = _copy_args(a)
-            da.lddy, da.w_bf16, da.flags = lddyb, ck.data_ptr(), 0
-            da.rowadd, da.residual, da.bias, da.x_bf16 = None, None, None, None
-            self._late.append(lambda da=da: setattr(da, "dy_bf16", self.sptr("dy_bf16")))
-            if dx_scratch is not None:
-                self.scratch(dx_scratch, x.rows * x.C)
-                da.ld_out = x.C
-                self._late.append(lambda da=da, n=dx_scratch: setattr(da, "out", self.sptr(n)))
-            else:
-                tgt = dx_into if dx_into is not None else x
-                gx = self.gradof(tgt)
-                da.out, da.ld_out = gx.ptr, gx.ld
-                it.writes.append((tgt, lambda init, da=da: setattr(da, "flags", 1 if init else 0), None))
+            da = _bwd_args(a)
+            da.lddy, da.w_bf16, da.x_bf16 = lddyb, ck.data_ptr(), None
+            self._late.append(lambda: setattr(da, "dy_bf16", self.sptr("dy_bf16")))
+            self._dgrad_target(it, da, x, dx_scratch, dx_into, "out", "ld_out", amax=False)
             self._rec(steps, lib.dp_conv2d_dgrad_bf16, da, "conv dgrad", info)
 
     GN_MAX_C = 1024      # channels one dp_groupnorm launch handles (256 threads x 4 channel slots); wider tensors are split by groups
@@ -883,7 +851,7 @@ class Plan:
             self._rec(it.steps, lib.dp_groupnorm_bwd, b, "gn bwd")
             if side_param:
                 self._rec(it.steps, lib.dp_groupnorm_bwd_param, b, "gn bwd param")
-                it.steps[-1].side = 2 if SIDE_WGRAD else 0     # only feeds Parameter.grad, like the weight gradients
+                it.steps[-1].side = 2     # only feeds Parameter.grad, like the weight gradients
 
         def resolve(init, parts=parts, gx=gx):
             if init:
@@ -1049,45 +1017,87 @@ class Plan:
         for t_, g_ in ((q, g_dq), (k, g_dk), (v, g_dv)):
             it.writes.append((t_, lambda init: None, lambda slot, g_=g_: setattr(g_, "amax_out", slot)))
 
+    # ------------------------------------------------------------------ network stem (shared by the DDPM and LDM builders)
+    def _padded(self, N: int, H: int, W: int, C_: int) -> View:
+        """Network input / output / context buffer, its pad channels zero: the pitch rounded to 4 floats is 16-byte aligned, so TMA can
+        read it and conv_in / conv_out run on the tensor-core path too."""
+        v = self.new(N, H, W, C_)
+        v.t.zero_()
+        return v
+
+    def _time_embedding(self, lin1: nn.Linear, lin2: nn.Linear, flip: bool, shift: float = 0):
+        """silu_temb = SiLU(lin2(SiLU(lin1(sinusoid(t_dev))))), the per-image input of every resnet's time_emb_proj (embeddings.py:22-62,
+        200-212).  flip: cos | sin halves; shift: the frequency denominator's offset."""
+        lib, B = self.lib, self.B
+        half = lin1.in_features // 2
+        self.freqs = sinusoidal_frequencies(lin1.in_features, shift).to(self.dev)
+        temb0 = self.new(B, 1, 1, 2 * half)
+        l1, s1 = self.new(B, 1, 1, lin1.out_features), self.new(B, 1, 1, lin1.out_features)
+        emb = self.new(B, 1, 1, lin2.out_features)
+        self.silu_temb = self.new(B, 1, 1, emb.C)
+
+        def silu(x: View, y: View):
+            n = B * x.ld      # flat extent incl. pitch padding (pads are never read as channels)
+            self._rec(self.fwd, lambda s: lib.dp_silu_fwd(x.ptr, y.ptr, n, s), what="silu")
+            if self.need_grad:
+                self._rec(self._bitem().steps, lambda s: lib.dp_silu_bwd(x.ptr, self.gradof(y).ptr, self.gradof(x).ptr, n, 0, s),
+                          what="silu bwd")
+        self._rec(self.fwd, lambda s: lib.dp_timestep_embedding(self.t_dev.data_ptr(), self.freqs.data_ptr(), temb0.ptr, B, half,
+                                                                1 if flip else 0, s), what="temb")
+        self.conv(temb0, lin1.weight, lin1.bias, l1, pad=0, need_dx=False)
+        silu(l1, s1)
+        self.conv(s1, lin2.weight, lin2.bias, emb, pad=0)
+        silu(emb, self.silu_temb)
+        if self.need_grad:
+            self.bwd[-1].steps[-1].join = True     # d silu(temb) is complete only when the side stream's time-embedding branches are
+
+    def _skips(self, shapes: List[Tuple[int, int, int]], cat_totals: List[int]) -> Callable[[], View]:
+        """Allocator of the skip tensors in forward order: skip i ((H, W, C) = shapes[i]) is the upper channel range of the
+        cat_totals[i]-channel buffer its up-path consumer reads as torch.cat([h, skip]), so the concatenation never copies."""
+        assert len(shapes) == len(cat_totals)
+        todo = iter(zip(shapes, cat_totals))
+
+        def new_skip() -> View:
+            (h, w, c), total = next(todo)
+            assert total - c > 0
+            return View(self.new(self.B, h, w, total).t, total - c, c)
+        return new_skip
+
+    def _upsample2x(self, x: View) -> View:
+        """Nearest-neighbour x2 upsampling of x, forward and backward; returns the upsampled tensor."""
+        lib = self.lib
+        up = self.new(x.N, 2 * x.H, 2 * x.W, x.C)
+        self._rec(self.fwd, lambda s: lib.dp_upsample2x_fwd(x.ptr, x.ld, up.ptr, up.ld, x.N, x.H, x.W, x.C, s), what="upsample")
+        self._alias_slot(up, x)
+        if self.need_grad:
+            it = self._bitem()
+            accf = [0]        # x.grad: = or +=, known once every writer of x.grad is
+            it.writes.append((x, lambda init: accf.__setitem__(0, 1 if init else 0), None))
+            self._rec(it.steps, lambda s: lib.dp_upsample2x_bwd(self.gradof(up).ptr, up.ld, self.gradof(x).ptr, self.gradof(x).ld,
+                                                                x.N, x.H, x.W, x.C, accf[0], s), what="upsample bwd")
+        return up
+
+    def _out_head(self, x: View, norm: nn.GroupNorm, conv: nn.Conv2d):
+        """self.y_out = conv(SiLU(norm(x))) (unet_2d.py:302-304), in a padded buffer whose gradient the loss fills."""
+        a = self.new(x.N, x.H, x.W, x.C)
+        g = self.gn(x, norm, a, silu=True)
+        if self.need_grad:
+            self.gn_bwd(g, x, norm, lambda: self.sptr("da"), x.C)
+        self.y_out = self._padded(self.B, self.H, self.W, conv.out_channels)
+        self.gradof(self.y_out).t.zero_()
+        self.conv(a, conv.weight, conv.bias, self.y_out, dx_scratch="da")
+
     # ------------------------------------------------------------------ whole network
     def _build(self):
         if hasattr(self.model, "input_blocks"):      # latent-diffusion UNetModel (ldm.py)
             return self._build_ldm()
-        m, lib = self.model, self.lib
-        B, H, W = self.B, self.H, self.W
+        m = self.model
+        H, W = self.H, self.W
         cfg = m.config
         self._setup_param_grads()
-        # ---- inputs + timestep embedding chain (embeddings.py:22-62, 200-212)
-        self.t_dev = torch.zeros(B, device=self.dev, dtype=torch.int64)
-        # network input / output live in buffers padded to a multiple of 4 channels (zero pad) so their pixel stride is
-        # 16-byte aligned: TMA can then read them and conv_in / conv_out run on the tensor-core path too
-        def padded(c):
-            t = torch.zeros((B, H, W, (c + 3) // 4 * 4), device=self.dev, dtype=torch.float32)
-            self._keep.append(t)
-            return View(t, 0, c)
-        self.x_in = padded(cfg.in_channels)
-        half = cfg.block_out_channels[0] // 2
-        self.freqs = sinusoidal_frequencies(cfg.block_out_channels[0], cfg.freq_shift).to(self.dev)
-        te = m.time_embedding
-        temb0 = self.new(B, 1, 1, 2 * half)
-        l1, s1 = self.new(B, 1, 1, te.linear_1.out_features), self.new(B, 1, 1, te.linear_1.out_features)
-        emb = self.new(B, 1, 1, te.linear_2.out_features)
-        self.silu_temb = self.new(B, 1, 1, emb.C)
-        self._rec(self.fwd, lambda s: lib.dp_timestep_embedding(self.t_dev.data_ptr(), self.freqs.data_ptr(), temb0.ptr, B, half,
-                                                                1 if cfg.flip_sin_to_cos else 0, s), what="temb")
-        self.conv(temb0, te.linear_1.weight, te.linear_1.bias, l1, pad=0, need_dx=False)
-        n1, n2 = B * l1.ld, B * emb.ld   # flat extents incl. pitch padding (pads are never read as channels)
-        self._rec(self.fwd, lambda s: lib.dp_silu_fwd(l1.ptr, s1.ptr, n1, s), what="silu")
-        if self.need_grad:
-            self._rec(self._bitem().steps, lambda s: lib.dp_silu_bwd(l1.ptr, self.gradof(s1).ptr, self.gradof(l1).ptr, n1, 0, s),
-                      what="silu bwd")
-        self.conv(s1, te.linear_2.weight, te.linear_2.bias, emb, pad=0)
-        self._rec(self.fwd, lambda s: lib.dp_silu_fwd(emb.ptr, self.silu_temb.ptr, n2, s), what="silu")
-        if self.need_grad:
-            self._rec(self._bitem().steps,
-                      lambda s: lib.dp_silu_bwd(emb.ptr, self.gradof(self.silu_temb).ptr, self.gradof(emb).ptr, n2, 0, s),
-                      what="silu bwd")
-            self.bwd[-1].steps[-1].join = True     # d silu(temb) is complete only when the side stream's time-embedding branches are
+        self.t_dev = torch.zeros(self.B, device=self.dev, dtype=torch.int64)
+        self.x_in = self._padded(self.B, H, W, cfg.in_channels)
+        self._time_embedding(m.time_embedding.linear_1, m.time_embedding.linear_2, cfg.flip_sin_to_cos, cfg.freq_shift)
 
         # ---- skip/concat geometry: every skip lives in the upper channel range of its consumer's concat buffer
         skip_shapes = []
@@ -1101,26 +1111,7 @@ class Plan:
                 ch = blk.downsamplers[0].conv.out_channels
                 hh, ww = hh // 2, ww // 2
                 skip_shapes.append((hh, ww, ch))
-        consumers = [r for blk in m.up_blocks for r in blk.resnets]
-        assert len(consumers) == len(skip_shapes)
-        cat_total = [0] * len(skip_shapes)
-        for j, r in enumerate(consumers):
-            cat_total[len(skip_shapes) - 1 - j] = r.norm1.num_channels
-        counter = [0]
-
-        def new_skip() -> View:
-            i = counter[0]
-            counter[0] += 1
-            hh_, ww_, c = skip_shapes[i]
-            buf = self.new(B, hh_, ww_, cat_total[i])
-            assert cat_total[i] - c > 0
-            return View(buf.t, cat_total[i] - c, c)
-
-        def h_half(skip: View) -> View:   # channels [0, C_h) of the skip's concat buffer
-            return View(skip.t, 0, skip.off)
-
-        def cat_of(skip: View) -> View:
-            return View(skip.t, 0, skip.off + skip.C)
+        new_skip = self._skips(skip_shapes, [r.norm1.num_channels for blk in m.up_blocks for r in blk.resnets][::-1])
 
         x = new_skip()
         self.conv(self.x_in, m.conv_in.weight, m.conv_in.bias, x, need_dx=False)
@@ -1179,31 +1170,11 @@ class Plan:
                 x = dest
             if blk.upsamplers is not None:
                 u: Upsample2D = blk.upsamplers[0]
-                up = self.new(x.N, 2 * x.H, 2 * x.W, x.C)
-                xx = x
-                self._rec(self.fwd, lambda s, xx=xx, up=up: lib.dp_upsample2x_fwd(xx.ptr, xx.ld, up.ptr, up.ld, xx.N, xx.H, xx.W, xx.C, s),
-                          what="upsample")
-                self._alias_slot(up, xx)
-                if self.need_grad:
-                    it = self._bitem()
-                    accf = [0]
-                    it.writes.append((xx, lambda init, accf=accf: accf.__setitem__(0, 1 if init else 0), None))
-                    self._rec(it.steps, lambda s, xx=xx, up=up, accf=accf: lib.dp_upsample2x_bwd(
-                        self.gradof(up).ptr, up.ld, self.gradof(xx).ptr, self.gradof(xx).ld, xx.N, xx.H, xx.W, xx.C, accf[0], s),
-                        what="upsample bwd")
                 dest = h_half(skips[-1])
-                self.conv(up, u.conv.weight, u.conv.bias, dest)
+                self.conv(self._upsample2x(x), u.conv.weight, u.conv.bias, dest)
                 x = dest
         assert not skips
-        # ---- out head (unet_2d.py:302-304)
-        a = self.new(x.N, x.H, x.W, x.C)
-        g = self.gn(x, m.conv_norm_out, a, silu=True)
-        if self.need_grad:
-            self.gn_bwd(g, x, m.conv_norm_out, lambda: self.sptr("da"), x.C)
-        self.y_out = padded(cfg.out_channels)
-        self.gradof(self.y_out).t.zero_()
-        self.conv(a, m.conv_out.weight, m.conv_out.bias, self.y_out, dx_scratch="da")
-
+        self._out_head(x, m.conv_norm_out, m.conv_out)
         self._finalize_build()
 
     def _finalize_build(self):
@@ -1323,39 +1294,15 @@ class Plan:
         """UNetModel.forward (openaimodel.py:710-742) as a static launch plan; same HBM conventions as the DDPM UNet (NHWC fp32 views,
         zero-copy skip concatenation, epilogue-fused bias / embedding row / residual)."""
         from types import SimpleNamespace as NS
-        m, lib = self.model, self.lib
+        m = self.model
         B, H, W = self.B, self.H, self.W
         cfg = m.config
         self._setup_param_grads()
         self.t_dev = torch.zeros(B, device=self.dev, dtype=torch.int64)
-
-        def padded(n, h, w, c):
-            t = torch.zeros((n, h, w, (c + 3) // 4 * 4), device=self.dev, dtype=torch.float32)
-            self._keep.append(t)
-            return View(t, 0, c)
-        self.x_in = padded(B, H, W, cfg.in_channels)
-        self.ctx_in = padded(B, 1, 1, cfg.context_dim)
-        mc = cfg.model_channels
-        half = mc // 2
-        self.freqs = sinusoidal_frequencies(mc, 0).to(self.dev)        # exp(-ln(1e4) i / half), util.py:160-162
-        temb0 = self.new(B, 1, 1, 2 * half)
-        te1, te2 = m.time_embed[0], m.time_embed[2]
-        l1, s1 = self.new(B, 1, 1, te1.out_features), self.new(B, 1, 1, te1.out_features)
-        emb = self.new(B, 1, 1, te2.out_features)
-        self.silu_temb = self.new(B, 1, 1, emb.C)
-        # cos | sin order (util.py:164) = the DDPM kernel with the halves flipped
-        self._rec(self.fwd, lambda s: lib.dp_timestep_embedding(self.t_dev.data_ptr(), self.freqs.data_ptr(), temb0.ptr, B, half, 1, s), what="temb")
-        self.conv(temb0, te1.weight, te1.bias, l1, pad=0, need_dx=False)
-        n1, n2 = B * l1.ld, B * emb.ld
-        self._rec(self.fwd, lambda s: lib.dp_silu_fwd(l1.ptr, s1.ptr, n1, s), what="silu")
-        if self.need_grad:
-            self._rec(self._bitem().steps, lambda s: lib.dp_silu_bwd(l1.ptr, self.gradof(s1).ptr, self.gradof(l1).ptr, n1, 0, s), what="silu bwd")
-        self.conv(s1, te2.weight, te2.bias, emb, pad=0)
-        self._rec(self.fwd, lambda s: lib.dp_silu_fwd(emb.ptr, self.silu_temb.ptr, n2, s), what="silu")
-        if self.need_grad:
-            self._rec(self._bitem().steps,
-                      lambda s: lib.dp_silu_bwd(emb.ptr, self.gradof(self.silu_temb).ptr, self.gradof(emb).ptr, n2, 0, s), what="silu bwd")
-            self.bwd[-1].steps[-1].join = True     # d silu(temb) is complete only when the side stream's time-embedding branches are
+        self.x_in = self._padded(B, H, W, cfg.in_channels)
+        self.ctx_in = self._padded(B, 1, 1, cfg.context_dim)
+        # exp(-ln(1e4) i / half) (util.py:160-162) in cos | sin order (util.py:164): the DDPM sinusoid with the halves flipped
+        self._time_embedding(m.time_embed[0], m.time_embed[2], flip=True)
 
         def as_resnet(rb):     # ResBlock (openaimodel.py:163-275) in the attribute vocabulary of Plan.resnet()
             sk = rb.skip_connection
@@ -1374,22 +1321,7 @@ class Plan:
                 elif hasattr(layer, "op"):
                     ch, hh, ww = layer.op.out_channels, hh // 2, ww // 2
             shapes.append((hh, ww, ch))
-        consumers = [blk[0] for blk in m.output_blocks]
-        assert len(consumers) == len(shapes)
-        cat_total = [0] * len(shapes)
-        for j, rb in enumerate(consumers):
-            cat_total[len(shapes) - 1 - j] = rb.in_layers[0].num_channels
-        counter = [0]
-
-        def new_skip() -> View:
-            i = counter[0]
-            counter[0] += 1
-            hh_, ww_, c = shapes[i]
-            buf = self.new(B, hh_, ww_, cat_total[i])
-            assert cat_total[i] - c > 0
-            return View(buf.t, cat_total[i] - c, c)
-        h_half = lambda skip: View(skip.t, 0, skip.off)
-        cat_of = lambda skip: View(skip.t, 0, skip.off + skip.C)
+        new_skip = self._skips(shapes, [blk[0].in_layers[0].num_channels for blk in m.output_blocks][::-1])
 
         def run_layers(layers, x: View, dest: View) -> View:
             """A TimestepEmbedSequential: the last layer writes `dest`, the others fresh buffers."""
@@ -1409,20 +1341,8 @@ class Plan:
                     y = dest
                     self.conv(x, layer.op.weight, layer.op.bias, y, stride=2, pad=1)
                 elif hasattr(layer, "conv"):      # Upsample: nearest x2 then 3x3 conv
-                    up = self.new(x.N, 2 * x.H, 2 * x.W, x.C)
-                    xx = x
-                    self._rec(self.fwd, lambda s, xx=xx, up=up: lib.dp_upsample2x_fwd(xx.ptr, xx.ld, up.ptr, up.ld, xx.N, xx.H, xx.W, xx.C, s),
-                              what="upsample")
-                    self._alias_slot(up, xx)
-                    if self.need_grad:
-                        it = self._bitem()
-                        accf = [0]
-                        it.writes.append((xx, lambda init, accf=accf: accf.__setitem__(0, 1 if init else 0), None))
-                        self._rec(it.steps, lambda s, xx=xx, up=up, accf=accf: lib.dp_upsample2x_bwd(
-                            self.gradof(up).ptr, up.ld, self.gradof(xx).ptr, self.gradof(xx).ld, xx.N, xx.H, xx.W, xx.C, accf[0], s),
-                            what="upsample bwd")
                     y = dest
-                    self.conv(up, layer.conv.weight, layer.conv.bias, y)
+                    self.conv(self._upsample2x(x), layer.conv.weight, layer.conv.bias, y)
                 else:
                     raise NotImplementedError(type(layer).__name__)
                 x = y
@@ -1449,13 +1369,7 @@ class Plan:
                 dest = self.new(cat.N, cat.H, cat.W, out_ch)
             x = run_layers(layers, cat, dest)
         assert not skips
-        a = self.new(x.N, x.H, x.W, x.C)
-        g = self.gn(x, m.out[0], a, silu=True)
-        if self.need_grad:
-            self.gn_bwd(g, x, m.out[0], lambda: self.sptr("da"), x.C)
-        self.y_out = padded(B, H, W, cfg.out_channels)
-        self.gradof(self.y_out).t.zero_()
-        self.conv(a, m.out[2].weight, m.out[2].bias, self.y_out, dx_scratch="da")
+        self._out_head(x, m.out[0], m.out[2])
         self._finalize_build()
 
     def load_context(self, context: torch.Tensor):
