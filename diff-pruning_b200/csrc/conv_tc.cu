@@ -15,8 +15,8 @@
 //
 // Kernels (warpgroup roles: sm90.cuh):
 //   conv_tc_ps_kernel     fprop / dgrad / NT GEMM: persistent (1 CTA per SM loops over (tile, K split) work items); each consumer
-//                         warpgroup splits its 64 rows of the raw fp32 A boxes IN PLACE into fp16 hi | lo' tiles, B = pre-split fp16
-//                         weights by TMA, 3 x 64 KB stages
+//                         thread loads its wgmma A fragments from the raw fp32 A boxes and splits them in registers (wgmma A from
+//                         registers, nothing written back), B = pre-split fp16 weights by TMA, 3 x 64 KB stages
 //   splitk_epilogue_kernel  fixed-order sum of the K splits + the epilogue (small-M launches)
 //   wgrad_tc_kernel       weight gradient: dY^T split in registers (wgmma A from registers), X split in place in shared memory
 //                         (MN-major B), 64-pixel stages, split-K over pixels
@@ -133,9 +133,11 @@ __device__ __forceinline__ void split1(float v, __half& h, __half& l) {
 }
 
 // ------------------------------------------------------------------------------------------------ persistent fprop / dgrad / NT GEMM
-// Stage = [A box k 0..31 | A box k 32..63 | b_hi | b_lo'] x 16 KB.  Consumer warpgroup c splits its tile rows 64c .. 64c+63 IN PLACE
-// (thread = row, raw box), then main += a_hi b_hi, corr += a_hi b_lo' + a_lo' b_hi per 16-element K step.  One wgmma group stays in
-// flight, so a warpgroup splits stage i+1 while the tensor cores run stage i.
+// Stage = [A box k 0..31 | A box k 32..63 | b_hi | b_lo'] x 16 KB.  Consumer warpgroup c owns tile rows 64c .. 64c+63: per 16-element
+// K step each thread loads its A fragment from the raw boxes, splits it in registers into a_hi | a_lo', and issues main += a_hi b_hi,
+// corr += a_hi b_lo' + a_lo' b_hi as one wgmma group.  One group stays in flight and two fragment sets alternate, so step k+1 is split
+// while the tensor cores run step k; only 16 fragment registers sit next to the 128 accumulators and the persistent loop's state, which
+// keeps ptxas from serialising the wgmma.
 constexpr int PS_STAGES = 3, PS_BN = 128;
 constexpr int PS_B_BYTES = PS_BN * BK * 2;
 constexpr int PS_STAGE_BYTES = 2 * A_BYTES + 2 * PS_B_BYTES;
@@ -240,8 +242,11 @@ conv_tc_ps_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constan
   setmaxnreg_inc<232>();
   const int c = wg - 1;                              // consumer warpgroup: tile rows 64c .. 64c + 63
   const int warp = tid >> 5, lane = tid & 31;
-  const int r = 64 * c + (tid & 63), h = tid >> 6;   // splitter task: row r, raw box h (K elements 32h .. 32h + 31 of the stage)
-  const uint32_t sw = (uint32_t)(r & 7);             // 128B swizzle: 16-byte chunk j of row r sits at chunk position j ^ (r & 7)
+  // A fragment of K step k (wgmma A from registers): rows 64c + 16 warp + lane/4 (+8), K elements 16k + 2 (lane%4) + {0, 1} (+8), i.e.
+  // raw box k/2, 16-byte chunk 4 (k%2) + (lane%4)/2 (+2), byte 8 (lane%2) of the chunk.  128B swizzle: chunk j of row r sits at j ^ (r & 7),
+  // and r & 7 = lane/4 for both rows, so chunk + 2 is position ^ 2 and row + 8 is 1 KB further; a warp's float2 loads are conflict free
+  const uint32_t frag_row = (uint32_t)(64 * c + 16 * warp + (lane >> 2)) * 128 + 8 * (lane & 1);
+  const uint32_t fsw = (uint32_t)(lane >> 2), fj = (uint32_t)((lane & 3) >> 1);
   const float sa = scale_up(amax_exponent(p.amax_a));
   // accumulators hold (s_a s_b) x the products: f1 * f2 undoes the two power-of-two operand scales (two factors: their product may underflow)
   const float f1 = scale_dn(amax_exponent(p.amax_a)), f2 = scale_dn(amax_exponent(p.amax_b)) * p.alpha;
@@ -251,46 +256,37 @@ conv_tc_ps_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constan
   for (int wi = blockIdx.x; wi < total_work; wi += gridDim.x) {
     const int tile = wi % total_tiles, it0 = (wi / total_tiles) * p.it_per_split, it1 = min(iters_per_tile, it0 + p.it_per_split);
     float acc[64], cor[64];
+    uint32_t fh[2][4], fl[2][4];              // fragment ring: K step k uses set k % 2 (4 steps per stage, so the set is static)
     int prev_s = 0;
     for (int it = it0; it < it1; ++it, ++g) {
       const int s = g % PS_STAGES;
       const uint32_t ph = (g / PS_STAGES) & 1u;
       mbar_wait(full_bar(s), ph);
-      uint8_t* a0 = smem + s * PS_STAGE_BYTES + r * 128;      // row r of the k 0..31 box  -> row r of a_hi
-      uint8_t* a1 = a0 + A_BYTES;                              // row r of the k 32..63 box -> row r of a_lo'
-      const uint8_t* src = h ? a1 : a0;
-      float4 v[8];
+      const uint8_t* stp = smem + s * PS_STAGE_BYTES + frag_row;
+      const uint32_t bst = sbase + s * PS_STAGE_BYTES + 2 * A_BYTES;
 #pragma unroll
-      for (int j = 0; j < 8; ++j) v[j] = *reinterpret_cast<const float4*>(src + ((j ^ sw) << 4));
-      named_sync(1 + c, 128);                                  // both halves of every row of this warpgroup have read it
-#pragma unroll
-      for (int m = 0; m < 4; ++m) {        // output chunk 4h + m = K elements 32h + 8m .. 32h + 8m + 7
-        const float4 x0 = v[2 * m], x1 = v[2 * m + 1];
-        uint4 hq, lq;
-        split2(x0.x * sa, x0.y * sa, hq.x, lq.x);
-        split2(x0.z * sa, x0.w * sa, hq.y, lq.y);
-        split2(x1.x * sa, x1.y * sa, hq.z, lq.z);
-        split2(x1.z * sa, x1.w * sa, hq.w, lq.w);
-        const uint32_t pos = (uint32_t)(((4 * h + m) ^ sw) << 4);
-        *reinterpret_cast<uint4*>(a0 + pos) = hq;
-        *reinterpret_cast<uint4*>(a1 + pos) = lq;
-      }
-      fence_proxy_async();
-      named_sync(1 + c, 128);                                  // the warpgroup's 64 rows are split
-      const uint32_t st = sbase + s * PS_STAGE_BYTES;
-      wgmma_fence();
-#pragma unroll
-      for (int k = 0; k < BK / 16; ++k) {      // one instruction = 16 fp16 along K = 32 bytes of every 128-byte row
-        const uint64_t a_hi = desc_k(st + c * 8192 + k * 32), a_lo = desc_k(st + A_BYTES + c * 8192 + k * 32);
-        const uint64_t b_hi = desc_k(st + 2 * A_BYTES + k * 32), b_lo = desc_k(st + 2 * A_BYTES + PS_B_BYTES + k * 32);
+      for (int k = 0; k < BK / 16; ++k) {      // one instruction = 16 fp16 along K = 32 bytes of every 128-byte B row
+        uint32_t (&ah)[4] = fh[k & 1];
+        uint32_t (&al)[4] = fl[k & 1];
+        const uint8_t* a = stp + (k >> 1) * A_BYTES;
+        const uint32_t pos = ((4u * (k & 1) + fj) ^ fsw) << 4;
+        const float2 v0 = *reinterpret_cast<const float2*>(a + pos), v1 = *reinterpret_cast<const float2*>(a + 1024 + pos);
+        const float2 v2 = *reinterpret_cast<const float2*>(a + (pos ^ 32u)), v3 = *reinterpret_cast<const float2*>(a + 1024 + (pos ^ 32u));
+        split2(v0.x * sa, v0.y * sa, ah[0], al[0]);
+        split2(v1.x * sa, v1.y * sa, ah[1], al[1]);
+        split2(v2.x * sa, v2.y * sa, ah[2], al[2]);
+        split2(v3.x * sa, v3.y * sa, ah[3], al[3]);
+        const uint64_t b_hi = desc_k(bst + k * 32), b_lo = desc_k(bst + PS_B_BYTES + k * 32);
         const uint32_t first = (it > it0 || k > 0) ? 1u : 0u;
-        wgmma_f16_n128<0, 0>(acc, a_hi, b_hi, first);
-        wgmma_f16_n128<0, 0>(cor, a_hi, b_lo, first);
-        wgmma_f16_n128<0, 0>(cor, a_lo, b_hi, 1u);
+        wgmma_fence();
+        wgmma_f16_n128_rs<0>(acc, ah, b_hi, first);
+        wgmma_f16_n128_rs<0>(cor, ah, b_lo, first);
+        wgmma_f16_n128_rs<0>(cor, al, b_hi, 1u);
+        wgmma_commit();
+        wgmma_wait<1>();                      // the step before has retired: its fragment set may be rewritten
+        // ... and at k = 0 that was the previous stage's last step: its B tiles are read, hand the stage back to the producer
+        if (k == 0 && it > it0 && lane == 0) mbar_arrive(empty_bar(prev_s));
       }
-      wgmma_commit();
-      wgmma_wait<1>();                        // the previous stage's MMAs have read their operands: hand it back to TMA
-      if (it > it0 && lane == 0) mbar_arrive(empty_bar(prev_s));
       prev_s = s;
     }
     wgmma_wait<0>();
