@@ -55,6 +55,11 @@ class TaylorArgs(C.Structure):
                 ("out_sq", vp), ("in_signed", vp), ("in_abs", vp), ("in_sq", vp)]
 
 
+class SsimArgs(C.Structure):
+    _fields_ = [("x", vp), ("y", vp), ("format", i32), ("N", i32), ("C", i32), ("H", i32), ("W", i32), ("win_size", i32),
+                ("win", C.c_double * 11), ("c1", C.c_double), ("c2", C.c_double), ("ssim_nc", vp), ("sse_n", vp)]
+
+
 class AdamArgs(C.Structure):
     _fields_ = [("n", i64), ("p", vp), ("g", vp), ("m", vp), ("v", vp), ("ema", vp), ("sumsq", vp),
                 ("max_norm", C.c_double), ("lr", C.c_double), ("beta1", C.c_double), ("beta2", C.c_double),
@@ -122,6 +127,7 @@ _SIGS = {
     "dp_pool3x3": (C.c_int, [vp, i64, vp, i64, i32, i32, i32, i32, i32, i32, i32, vp, vp]),
     "dp_global_mean": (C.c_int, [vp, i64, vp, i64, i32, i32, i32, i32, vp]),
     "dp_feature_moments": (C.c_int, [vp, i64, i64, i32, vp, vp, vp, vp]),
+    "dp_ssim": (C.c_int, [C.POINTER(SsimArgs), vp]),
 }
 EXPORTS = tuple(_SIGS)
 

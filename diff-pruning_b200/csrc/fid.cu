@@ -2,6 +2,7 @@
 // the global mean, and fp64 feature moments.  Every sum runs in a fixed order, so features and moments are run-to-run identical.
 #include <math.h>
 #include "common.cuh"
+#include "image_src.cuh"
 
 namespace {
 constexpr int NT = 256;
@@ -12,17 +13,9 @@ static inline int nblocks(long long n, int cap = DP_NUM_SMS * 32) {
   return (int)b;
 }
 
-// One source value in [0, 1], as the reference's input tensor holds it.  The explicit _rn intrinsics keep nvcc from contracting the
-// PNG quantisation into FMAs, which would round differently from the numpy / PIL chain it restates.
+// One RGB source value in [0, 1] (image_src.cuh)
 __device__ __forceinline__ float fid_src(const void* src, int u8, int quantize, int n, int c, int h, int w, int Hs, int Ws) {
-  if (u8) {
-    const uint8_t u = static_cast<const uint8_t*>(src)[(((long long)n * Hs + h) * Ws + w) * 3 + c];
-    return __fdiv_rn((float)u, 255.0f);
-  }
-  const float x = static_cast<const float*>(src)[(((long long)n * 3 + c) * Hs + h) * Ws + w];
-  if (!quantize) return x;
-  const float v = fminf(fmaxf(__fadd_rn(__fmul_rn(x, 0.5f), 0.5f), 0.0f), 1.0f);
-  return __fdiv_rn(rintf(__fmul_rn(v, 255.0f)), 255.0f);
+  return dp_image_src(src, u8, quantize, n, c, h, w, 3, Hs, Ws);
 }
 
 // one thread per output pixel (all three channels)

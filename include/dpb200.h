@@ -381,6 +381,35 @@ int dp_global_mean(const float* x, int64_t ldx, float* y, int64_t ldy, int32_t N
  * run-to-run identical, and moments about the same shift from several batches (or devices) are plain sums. */
 int dp_feature_moments(const float* f, int64_t ld, int64_t rows, int32_t D, const float* shift, double* sum, double* sxx, dp_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * SSIM evaluation (ssim.cu): pytorch_msssim.ssim's per-channel SSIM (compute_ssim.py) and the per-image squared error, for N image pairs.
+ * ------------------------------------------------------------------------------------------------ */
+#define DP_SSIM_WIN 11
+enum {
+  DP_SSIM_U8_NHWC = 0,      /* uint8 NHWC [N][H][W][C] (decoded image files), value u / 255 correctly rounded, as ToTensor gives it */
+  DP_SSIM_F32_NCHW = 1,     /* fp32 NCHW [N][C][H][W], as given */
+  DP_SSIM_F32_NCHW_PNG = 2  /* fp32 NCHW DDIM samples in [-1, 1] taken through the sampler's PNG write, as dp_fid_input's `quantize` */
+};
+typedef struct dp_ssim_args {
+  const void* x; const void* y;   /* the two images of each pair, both in `format` */
+  int32_t format;                 /* DP_SSIM_* */
+  int32_t N, C, H, W;             /* H, W >= win_size */
+  int32_t win_size;               /* must be DP_SSIM_WIN */
+  double win[DP_SSIM_WIN];        /* separable window taps, host-computed (pytorch_msssim builds them in fp32; those sum to 1 only to
+                                     ~1e-7, which moves SSIM by up to ~1e-5 on images with large means — fp64 taps follow the exact
+                                     definition) */
+  double c1, c2;                  /* (K1 data_range)^2, (K2 data_range)^2 */
+  double* ssim_nc;                /* out [N][C]: mean of the SSIM map per image and channel */
+  double* sse_n;                  /* out [N]: sum over c, h, w of (x - y)^2, the difference taken in fp32 and squared exactly in fp64 */
+} dp_ssim_args;
+/* The window runs along H, then along W, "valid" (the map is (H - win_size + 1) x (W - win_size + 1)).  The five filtered moments
+ * mu_x, mu_y, E[x^2], E[y^2], E[xy] are accumulated in fp64 from exact fp64 products of the fp32 inputs, and the map
+ *   ((2 mu_x mu_y + c1) / (mu_x^2 + mu_y^2 + c1)) ((2 s_xy + c2) / (s_x^2 + s_y^2 + c2)),  s_x^2 = E[x^2] - mu_x^2, ...
+ * is formed in fp64.  One fixed set of blocks per image and fixed summation orders, no atomics: results are run-to-run identical and an
+ * image's results do not depend on the rest of the batch.  DP_ERR_SHAPE for H or W < win_size, DP_ERR_UNSUPPORTED for another window
+ * size or format. */
+int dp_ssim(const dp_ssim_args* a, dp_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -15,6 +15,7 @@ Outputs (all small, committed):
     tests/golden/finetune_tiny.pt  2 finetune steps on TINY (Adam + clip + EMA), dropout 0
     tests/golden/ddim_tiny.pt      DDIMPipeline samples (uniform/eta 0/10 steps, quad/eta 0.5/7 steps) on TINY
     tests/golden/fid_*             FID Inception fixtures (gen_fid): weight-file layout, features of seeded weights, Frechet cases
+    tests/golden/ssim_ref.pt       SSIM fixtures (gen_ssim): uint8 image pairs and utils_image.py's per-channel / per-image SSIM
 """
 import argparse
 import hashlib
@@ -629,13 +630,56 @@ def gen_fid():
     print("fid frechet", [c.get("fid", c.get("error")) for c in cases])
 
 
+def gen_ssim():
+    """SSIM fixtures from the UNMODIFIED ldm_exp/ldm/modules/image_degradation/utils_image.py (fp64 NumPy + cv2: 11-tap Gaussian,
+    sigma 1.5, valid region, C1 = (0.01 * 255)^2, C2 = (0.03 * 255)^2), loaded by file path so that ldm/__init__ is not imported.
+    Writes ssim_ref.pt: a list of seeded uint8 HWC image pairs, each with the reference's per-channel ssim() and calculate_ssim()."""
+    import importlib.util
+    import numpy as np
+    path = os.path.join(ref_shim.REF, "ldm_exp", "ldm", "modules", "image_degradation", "utils_image.py")
+    spec = importlib.util.spec_from_file_location("ref_utils_image", path)
+    ui = importlib.util.module_from_spec(spec)
+    spec.loader.exec_module(ui)
+    rng = np.random.default_rng(4)
+
+    def u8(a):
+        return np.clip(np.rint(a), 0, 255).astype(np.uint8)
+
+    def smooth(h, w):
+        yy, xx = np.meshgrid(np.linspace(0, 1, h), np.linspace(0, 1, w), indexing="ij")
+        ph = rng.uniform(0, 2 * np.pi, 3)
+        return np.stack([128 + 90 * np.sin(2 * np.pi * (1.3 * xx + 0.7 * yy) + ph[c]) * np.cos(3 * yy + c) for c in range(3)], -1)
+
+    pairs = []
+    noise = rng.integers(0, 256, (32, 32, 3))
+    pairs.append(("noise", u8(noise), u8(rng.integers(0, 256, (32, 32, 3)))))
+    s = smooth(32, 32)
+    pairs.append(("smooth_vs_noisy", u8(s), u8(s + rng.normal(0, 4, s.shape))))
+    flat = np.full((32, 32, 3), 100.0)
+    pairs.append(("flat_vs_flat_plus_1", u8(flat), u8(flat + 1)))     # zero variance: the moments cancel exactly down to C2
+    pairs.append(("inverted", u8(s), u8(255 - s)))
+    pairs.append(("identical", u8(noise), u8(noise)))
+    s = smooth(48, 40)
+    pairs.append(("nonsquare_48x40", u8(s), u8(s + rng.normal(0, 8, s.shape))))
+    s = smooth(256, 256)
+    pairs.append(("smooth_256", u8(s), u8(s + rng.normal(0, 6, s.shape))))
+    out = []
+    for name, x, y in pairs:
+        per_c = [float(ui.ssim(x[:, :, c], y[:, :, c])) for c in range(3)]
+        out.append({"name": name, "x": torch.from_numpy(x), "y": torch.from_numpy(y), "ssim_c": torch.tensor(per_c, dtype=torch.float64),
+                    "ssim": float(ui.calculate_ssim(x, y))})
+        print("ssim", name, x.shape, per_c, out[-1]["ssim"])
+    torch.save(out, os.path.join(OUT, "ssim_ref.pt"))
+    print("ssim_ref.pt", os.path.getsize(os.path.join(OUT, "ssim_ref.pt")))
+
+
 if __name__ == "__main__":
     ap = argparse.ArgumentParser()
     ap.add_argument("--skip-cfg1", action="store_true")
     ap.add_argument("--only", default=None)
     a = ap.parse_args()
     torch.set_num_threads(os.cpu_count())
-    jobs = {"fid": gen_fid, "ldm_tiny": gen_ldm_tiny, "exp_importance": gen_exp_importance, "ref_pickle": gen_ref_pickle, "lsun_struct": gen_lsun_struct, "lr": gen_lr, "ckpt": gen_ckpt, "ddim": gen_ddim, "tiny": gen_tiny, "blocks": gen_blocks, "finetune": gen_finetune, "cifar_fwd": gen_cifar_fwd,
+    jobs = {"ssim": gen_ssim, "fid": gen_fid,"ldm_tiny": gen_ldm_tiny, "exp_importance": gen_exp_importance, "ref_pickle": gen_ref_pickle, "lsun_struct": gen_lsun_struct, "lr": gen_lr, "ckpt": gen_ckpt, "ddim": gen_ddim, "tiny": gen_tiny, "blocks": gen_blocks, "finetune": gen_finetune, "cifar_fwd": gen_cifar_fwd,
             "cfg1_s3": gen_cfg1_s3, "cfg3_s3": gen_cfg3_s3, "cfg1": gen_cfg1}
     for name, fn in jobs.items():
         if a.only and name != a.only:
