@@ -33,6 +33,9 @@ Step = Callable[[int], None]
 
 _SM_COUNT = 132            # H100 SXM; the wgrad kernel runs one CTA per SM (192 KB of shared memory)
 _WGRAD_CTA_OVERHEAD = 8    # per-CTA prologue + pipeline fill + register->workspace epilogue, in units of one 64-pixel stage
+_WGRAD_MAX_CHUNKS = 147    # 64-pixel chunks one wgrad CTA may walk (9408 pixels): the tensor core truncates every fp32 accumulator update,
+                           # so a CTA's drift grows linearly with its chain of pixels / 16 updates; past ~600 updates it approaches the
+                           # error of a dropped lo' correction term and the fp32-grade claim can no longer be checked (tests/launch_census.py)
 
 
 def _wgrad_splits(tiles, chunks):
@@ -40,12 +43,14 @@ def _wgrad_splits(tiles, chunks):
     One CTA per SM, so the launch runs in ceil(grid / 132) strict waves: pick the split count whose modelled time
     waves x (overhead + chunks per CTA) is smallest (ties: fewer splits = smaller workspace), so a grid never overshoots a
     wave boundary by a few CTAs (530 CTAs would cost a fifth, almost empty, wave) and no trailing split is empty.
-    The search stops at 8 waves' worth of CTAs."""
+    The search stops at 8 waves' worth of CTAs.  A CTA walks at most _WGRAD_MAX_CHUNKS chunks whenever a split count within the search
+    allows it."""
     hi = max(1, min(chunks, max(2, (8 * _SM_COUNT) // tiles)))
+    cap = _WGRAD_MAX_CHUNKS if -(-chunks // hi) <= _WGRAD_MAX_CHUNKS else chunks
     best = None
     for sp in range(1, hi + 1):
         cps = -(-chunks // sp)
-        if cps * (sp - 1) >= chunks:                 # would leave the last split empty: same as a smaller split count
+        if cps * (sp - 1) >= chunks or cps > cap:    # an empty last split (same as a smaller split count), or too long a chain
             continue
         cost = -(-(tiles * sp) // _SM_COUNT) * (_WGRAD_CTA_OVERHEAD + cps)
         if best is None or cost < best[0]:

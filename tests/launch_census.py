@@ -1,0 +1,164 @@
+"""Error model, chain lengths and launch dedup key of the launch census (test_launch_census_gpu.py, checked on the host by
+test_launch_census_host.py).
+
+Error model of a product-sum output y_i = sum_k a_k b_k computed by the tensor-core kernels:
+  * operands: the 3 x fp16 split keeps 22 bits of each operand and drops lo' * lo' (conv_tc.cu), so every product carries a relative
+    error of a few 2^-22 with a random sign; over the sum that is a few 2^-22 * s_i, s_i = sqrt(sum_k (a_k b_k)^2).
+  * accumulation: wgmma adds each 16-deep block of products into the fp32 accumulator with a TRUNCATING rounding: every one of the L
+    updates of one output loses less than one ulp of the partial sum, ulp(v) <= 2^-23 |v|, and these errors all have the sign of the
+    partial sum, so they add up linearly to < 2^-23 L mean_j |partial sum j|.  For the random-sign operands of the census the mean
+    magnitude of the partial sums is about 0.53 s_i, s_i = sqrt(sum_k (a_k b_k)^2), and stays below 1.5 s_i: BETA = 2 * 1.5 = 3.
+  * epilogue: bias / per-image row / residual / the old value (+=) each cost at most one fp32 rounding of the running value.
+Hence  |y^ - y| <= (ALPHA + BETA * L) * 2^-24 * s_i + 2^-23 * sum|epilogue terms|.
+ALPHA = 64 covers the operand split (a few 2^-22 s_i with its tail) and the final fp32 rounding of the output.  The bf16 tier is held
+to the same bound against fp64 math on the bf16-rounded operands (its products are exact, only the accumulation rounds).
+
+The bound keeps its teeth only while the accumulation term stays below the error of a dropped lo' correction term (about 2^-12.3 s_i):
+every tensor-core launch of the census must have L <= L_MAX, the longest chain at which test_launch_census_host.py shows that the
+split with one correction term dropped violates the bound on most outputs.
+
+Fixed-order fp32 sums with round-to-nearest (column sums, GroupNorm statistics, loss / norm reductions) are held to
+SUM_ALPHA * 2^-24 * s + 8 * sqrt(n) * 2^-24 * s (sum_bound): the n rounding errors are independent, zero-mean and each below 2^-24 of a
+partial sum of order s, so their total is of order sqrt(n) 2^-24 s; 8 standard deviations is never reached by chance, while dropping a
+single term of typical size s / sqrt(n) exceeds it for every n < 2^21.
+"""
+from __future__ import annotations
+
+import ctypes as C
+import math
+
+import torch
+
+U = 2.0 ** -24
+ALPHA, BETA = 64.0, 3.0
+L_MAX = 640
+SUM_ALPHA = 16.0
+
+
+def chain_fprop(taps: int, kg: int, ksplit: int = 1) -> int:
+    """fp32 accumulator updates of one output of a fprop / dgrad / NT-GEMM launch: taps x ceil(Kg / 64) pipeline stages of 4 wgmma
+    k-steps each, divided over ksplit K splits (splitk_count), plus the fixed-order sum of the splits."""
+    return -(-taps * -(-kg // 64) * 4 // ksplit) + ksplit
+
+
+def chain_wgrad(pixels_per_cta: int, splits: int) -> int:
+    """fp32 accumulator updates of one weight-gradient element: one per 16 pixels a CTA walks, plus the fixed-order reduce of the
+    splits."""
+    return -(-pixels_per_cta // 16) + splits
+
+
+def wgrad_pixels_per_cta(rows: int, splits: int) -> int:
+    """Pixels one CTA of dp_conv2d_wgrad walks: the kernel cuts the rows into 64-pixel chunks and gives each split ceil(chunks / splits)."""
+    chunks = max(1, rows // 64)
+    return -(-chunks // splits) * 64
+
+
+def product_bound(s: torch.Tensor, L: int, epi_abs=None) -> torch.Tensor:
+    """Element-wise bound of a product-sum output (see the module docstring); s and epi_abs in float64."""
+    b = (ALPHA + BETA * L) * U * s
+    if epi_abs is not None:
+        b = b + 2 * U * epi_abs
+    return b
+
+
+def sum_bound(s: torch.Tensor, n: int) -> torch.Tensor:
+    """Element-wise bound of a fixed-order fp32 sum of n terms whose squares sum to s^2 (see the module docstring)."""
+    return (SUM_ALPHA + 8.0 * math.sqrt(n)) * U * s
+
+
+def splitk_count(need_floats: int, rows: int, cols: int, stages: int) -> int:
+    """K splits of a fprop / dgrad launch from its split-K workspace size, which holds ksplit x [M tiles x 128][N tiles x 128] floats
+    (the launch's `stages` = taps x ceil(Kg / 64) pipeline stages are split at most 16 ways, at least 4 stages per split)."""
+    if need_floats <= 0:
+        return 1
+    ks = need_floats // ((-(-rows // 128) * 128) * (-(-cols // 128) * 128))
+    return max(1, min(ks, 16, stages // 4))
+
+
+def violations(got: torch.Tensor, ref: torch.Tensor, bound: torch.Tensor, limit: int = 8):
+    """(worst err / bound, coordinates of up to `limit` elements where |got - ref| > bound, or where got is not finite)."""
+    err = (got.double() - ref.double()).abs()
+    bad = ~(err <= bound)
+    ratio = (err / bound.clamp_min(1e-300))
+    worst = float(ratio.max()) if ratio.numel() else 0.0
+    if not bool(torch.isfinite(got).all()):
+        worst = math.inf
+    coords = [tuple(int(c) for c in idx) for idx in bad.nonzero()[:limit].tolist()]
+    return worst, coords
+
+
+def argkinds(name: str):
+    """'p' / 'i' / 'f' / 's' (struct) per argument of an exported entry point, from its ctypes signature; the trailing stream dropped."""
+    from diff_pruning_b200 import _lib as L
+    kinds = []
+    for t in list(L._SIGS[name][1])[:-1]:
+        if t is C.c_void_p:
+            kinds.append("p")
+        elif t in (C.c_float, C.c_double):
+            kinds.append("f")
+        elif isinstance(t, type) and issubclass(t, C._Pointer):
+            kinds.append("s")
+        else:
+            kinds.append("i")
+    return kinds
+
+
+def _ptr_key(v, esz: int = 4):
+    """A pointer's part of the key: NULL or not, and its 16-byte alignment phase in elements of `esz` bytes (the element offset of a
+    view mod 16 / esz)."""
+    return None if not v else (int(v) % 16) // esz
+
+
+BF16_FIELDS = {"x_bf16", "dy_bf16", "w_bf16", "y_bf16"}   # 2-byte elements in the argument structs
+
+
+def struct_key(s: C.Structure):
+    out = []
+    for name, t in s._fields_:
+        v = getattr(s, name)
+        if t is C.c_void_p:
+            out.append((name, _ptr_key(v, 2 if name in BF16_FIELDS else 4)))
+        elif hasattr(v, "__len__"):
+            out.append((name, tuple(v)))
+        else:
+            out.append((name, v))
+    return tuple(out)
+
+
+def launch_key(name: str, kinds, args):
+    """Dedup key of one captured call: the entry point, every integer / float field or argument (extents, ld, flags, splits ...),
+    and for every pointer whether it is set and its 16-byte phase."""
+    parts = [name]
+    for k, v in zip(kinds, args):
+        if k == "s":
+            parts.append(struct_key(v))
+        elif k == "p":
+            parts.append(_ptr_key(v, 2))      # plain pointer arguments: the finer phase (bf16 / fp16 buffers among them)
+        else:
+            parts.append(v)
+    return tuple(parts)
+
+
+# ---------------------------------------------------------------------------------------------------- host emulation of the split
+def split_h(v: torch.Tensor):
+    """The 3 x fp16 split of conv_tc.cu on the host: (hi, lo', scale) with s*v = hi + lo' / 2^11, |s*v| < 2^14 (float64 results)."""
+    e = math.floor(math.log2(float(v.abs().max()))) + 1
+    s = 2.0 ** (14 - e)
+    sv = v.double() * s
+    hi = sv.half().double()
+    lo = ((sv - hi) * 2048).half().double()
+    return hi, lo, s
+
+
+def c5_model():
+    """cin256-v2 as bench.py builds it: seed-0 init, the zero-initialised convolutions re-drawn (a fresh LDM UNet outputs exactly 0).
+    Returns (model, config)."""
+    from diff_pruning_b200 import ldm
+    cfg = ldm.CIN256_V2_CONFIG
+    torch.manual_seed(0)
+    m = ldm.UNetModel(**cfg)
+    g = torch.Generator().manual_seed(5)
+    for p in m.parameters():
+        if p.dim() > 1 and float(p.detach().abs().sum()) == 0:
+            p.data.copy_(torch.randn(p.shape, generator=g) * 0.02)
+    return m, cfg

@@ -190,8 +190,10 @@ def test_conv_tc_fprop_dgrad(lib, N, Cin, H, W, K, R, ldx, ldy):
     # wgrad (MN-major operands, both split in-kernel), deterministic split-K + reduce into dW (+=)
     pix_chunks = max(1, N * H * W // 64)
     # the tensor core adds every K-block of products into the fp32 accumulator with a truncating rounding, so ONE CTA walking tens of
-    # thousands of pixels drifts by a few 1e-5 (7.5e-5 at 32768 pixels); the engine's wave-aware split-K keeps a CTA at <= 8192 pixels and
-    # so do the large cases here (the small ones keep their 1 / 3 / 7-way splits incl. the trailing EMPTY split of 7 over 16 chunks)
+    # thousands of pixels drifts by a few 1e-5 (7.5e-5 at 32768 pixels).  The engine's wave-aware split-K does not cap a CTA's pixels (up
+    # to 18752 in C1 at batch 128); test_launch_census_gpu.py replays the engine's own split counts against a chain-length-aware bound.
+    # The large cases here keep a CTA at <= 8192 pixels (the small ones keep their 1 / 3 / 7-way splits incl. the trailing EMPTY split
+    # of 7 over 16 chunks)
     base = max(1, -(-(N * H * W) // 8192))
     for splits in sorted({base, min(3 * base, pix_chunks), min(7 * base, pix_chunks)} if base > 1 else {1, min(3, pix_chunks), min(7, pix_chunks)}):
         ws = torch.full((splits * K * R * R * Cin,), float("nan"), device="cuda")

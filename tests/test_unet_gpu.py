@@ -582,6 +582,42 @@ def test_ldm_unet_two_accumulated_passes_vs_reference():
     assert worst_grad_err(((k, p.grad) for k, p in m.named_parameters()), G["grads"]) < 1e-4
 
 
+def test_ldm_cin256_v2_full_width_two_accumulated_passes_vs_fp64_oracle():
+    """C5 at its real widths (cin256-v2, 400.9 M parameters: 192-960 channels, 6 / 18 / 30 channels per GroupNorm group, concatenations
+    up to 1920 channels, attention over 1024 tokens on the tensor-core NT GEMM, LayerNorm at 192-960, GEGLU inner widths up to 3840,
+    context_dim 512), built as bench.py builds it, batch 2 of 3x64x64 latents: two accumulated Taylor passes (t = 7, 400) against
+    oracle/ldm_oracle.py evaluated in float64 on the host, with the same criteria as the ldm_tiny test."""
+    from launch_census import c5_model
+    from oracle import ldm_oracle as lorc
+    from diff_pruning_b200 import ldm
+    m, cfg = c5_model()
+    B = 2
+    ctx = torch.randn(B, 1, cfg["context_dim"], generator=torch.Generator().manual_seed(9))
+    clean, noise = inputs(B, 64)
+    sd = {k: v.detach().double().requires_grad_(True) for k, v in m.state_dict().items()}
+    ac = lorc.alphas_cumprod()
+    torch.set_num_threads(min(32, torch.get_num_threads()))
+    m = m.cuda()
+    m.zero_grad()
+    sc = TaylorScorer(m, clean.cuda(), noise.cuda(), alphas_cumprod=ldm.ldm_alphas_cumprod(), use_graph=False, context=ctx.cuda())
+    for tt in (7, 400):
+        t = torch.full((B,), tt, dtype=torch.long)
+        out_ref = lorc.unet_forward(sd, cfg, lorc.q_sample(ac, clean.double(), noise.double(), t), t, ctx.double())
+        loss_ref = F.mse_loss(out_ref, noise.double())
+        loss_ref.backward()
+        loss = sc.step(tt).item()
+        eps = max_rel(sc.plan.output_nchw(), out_ref)
+        print(f"C5 t={tt}: loss {loss:.9f} (fp64 oracle {loss_ref.item():.9f}), eps_hat max-rel {eps:.2e}")
+        assert loss == pytest.approx(loss_ref.item(), rel=5e-6), tt
+        assert eps < 1e-4, tt
+    ref = {k: v.grad for k, v in sd.items()}
+    worst = worst_grad_err(((k, p.grad) for k, p in m.named_parameters()), ref)
+    print(f"C5 worst gradient error {worst:.2e}")
+    assert worst < 1e-4, worst
+    zero = [k for k, p in m.named_parameters() if float(ref[k].abs().max()) == 0.0]
+    assert zero and all(float(dict(m.named_parameters())[k].grad.abs().max()) == 0.0 for k in zero), zero
+
+
 @pytest.mark.parametrize("family", ["unet2d_c1", "unet2d_lsun_block", "ldm_tiny"])
 def test_amax_slots_bound_their_operands(family):
     """Every tensor-core launch scales its operands by the power of two taken from an amax slot.  Most slots are filled by the kernel
