@@ -28,6 +28,7 @@ import ctypes as C
 import math
 
 import torch
+import torch.nn.functional as F
 
 U = 2.0 ** -24
 ALPHA, BETA = 64.0, 3.0
@@ -73,6 +74,119 @@ def splitk_count(need_floats: int, rows: int, cols: int, stages: int) -> int:
         return 1
     ks = need_floats // ((-(-rows // 128) * 128) * (-(-cols // 128) * 128))
     return max(1, min(ks, 16, stages // 4))
+
+
+def pick_ksplit(tiles: int, iters: int, num_sms: int):
+    """conv_tc.cu's pick_ksplit: (K splits, pipeline stages per split) of a persistent-kernel launch with `tiles` output tiles of `iters`
+    stages each.  No split when the tiles already cover half the SMs or there are fewer than 8 stages; otherwise enough work items to
+    fill the SMs, at least 4 stages per split, at most 16 splits, and no empty split."""
+    if tiles * 2 > num_sms or iters < 8:
+        return 1, iters
+    ks = min(num_sms // tiles, iters // 4, 16)
+    if ks < 2:
+        return 1, iters
+    ips = -(-iters // ks)
+    return -(-iters // ips), ips
+
+
+def general_split(N: int, P: int, Q: int, K: int, C: int, R: int, S: int, num_sms: int):
+    """(K splits, stages per split) of a general-geometry fprop (conv_tc_ps_kernel<true>): ceil(N P Q / 128) x ceil(K / 128) output
+    tiles of R S ceil(C / 64) stages."""
+    tiles = -(-(N * P * Q) // 128) * -(-K // 128)
+    return pick_ksplit(tiles, R * S * -(-C // 64), num_sms)
+
+
+def chain_general(ksplit: int, stages_per_split: int) -> int:
+    """fp32 accumulator updates of one output of a general-geometry fprop: 4 wgmma k-steps per stage of its split, plus the fixed-order
+    sum of the splits."""
+    return 4 * stages_per_split + ksplit
+
+
+# ---------------------------------------------------------------------------------------------------- evaluation path (FID, DDIM)
+U53 = 2.0 ** -53
+
+
+def bilinear_coords(n_src: int, n_dst: int, half_pixel: bool = True):
+    """Source rows of a bilinear resize to n_dst, as torch's align_corners=False rule forms them in fp32: scale = n_src / n_dst,
+    r = max(scale (dst + 0.5) - 0.5, 0), i0 = trunc(r), i1 = i0 + 1 except on the last row, l1 = r - i0, l0 = 1 - l1 (fp32).
+    half_pixel=False drops the half-pixel offset (r = scale dst).  Returns (i0, i1, l0, l1, slack): the weights in float64 and
+    slack, two ulps of scale (dst + 0.5), a bound on how far a contracted (fma) evaluation of r can move the weights."""
+    f = torch.float32
+    d = torch.arange(n_dst, dtype=f)
+    scale = torch.tensor(float(n_src), dtype=f) / torch.tensor(float(n_dst), dtype=f)
+    prod = scale * (d + 0.5) if half_pixel else scale * d
+    r = (prod - 0.5).clamp_min(0.0) if half_pixel else prod
+    i0 = r.long()
+    i1 = torch.where(i0 < n_src - 1, i0 + 1, i0)
+    l1 = r - i0.to(f)
+    l0 = 1.0 - l1
+    return i0, i1, l0.double(), l1.double(), 2.0 ** -22 * prod.double()
+
+
+def bilinear_ref(src: torch.Tensor, Ho: int, Wo: int, half_pixel: bool = True):
+    """(ref, bound) of a bilinear resize of src [N, C, Hs, Ws] (float64: the values the kernel reads) to Ho x Wo, interpolated in fp64
+    from the fp32 weights of bilinear_coords.  The kernel's fp32 interpolation is a convex combination of four values, six roundings:
+    8 2^-24 of the largest neighbour covers it.  A weight moved by `slack` moves the result by at most slack x the largest jump between
+    neighbouring source values, bounded by 2 max|src| of the image channel (the moved weight may select the next source row)."""
+    N, Cc, Hs, Ws = src.shape
+    h0, h1, a0, a1, sh = bilinear_coords(Hs, Ho, half_pixel)
+    w0, w1, b0, b1, sw = bilinear_coords(Ws, Wo, half_pixel)
+    dev = src.device
+    h0, h1, w0, w1 = (t.to(dev) for t in (h0, h1, w0, w1))
+    A0, A1, sh = (t.to(dev).view(-1, 1) for t in (a0, a1, sh))
+    B0, B1, sw = (t.to(dev).view(1, -1) for t in (b0, b1, sw))
+    rows0, rows1 = src[:, :, h0], src[:, :, h1]
+    v00, v01, v10, v11 = rows0[..., w0], rows0[..., w1], rows1[..., w0], rows1[..., w1]
+    ref = A0 * (B0 * v00 + B1 * v01) + A1 * (B0 * v10 + B1 * v11)
+    vmax = torch.stack([v00.abs(), v01.abs(), v10.abs(), v11.abs()]).amax(0)
+    smax = src.abs().amax((2, 3), keepdim=True)
+    return ref, 8 * U * vmax + 2 * smax * (sh + sw)
+
+
+def avgpool_ref(x: torch.Tensor, stride: int, pad: int):
+    """(ref, bound) of the 3 x 3 average pool that does not count padding (count_include_pad=False) of x [N, C, H, W] float64: the
+    fixed-order fp32 sum of the n <= 9 taps inside the image (sum_bound), then one rounding of the division by n."""
+    ref = F.avg_pool2d(x, 3, stride, pad, count_include_pad=False)
+    n = F.avg_pool2d(torch.ones_like(x[:1, :1]), 3, stride, pad, count_include_pad=True) * 9          # taps inside the image
+    s = (F.avg_pool2d(x * x, 3, stride, pad, count_include_pad=False) * n).sqrt()
+    return ref, (SUM_ALPHA + 8.0 * 3.0) * U * s / n + 2 * U * ref.abs()
+
+
+def global_mean_ref(x: torch.Tensor):
+    """(ref, bound) of the mean over H x W of x [N, C, H, W] float64 as dp_global_mean forms it: an fp64 sum of the H W fp32 terms
+    ((H W + 4) 2^-53 sum|x|), one fp64 division and one rounding to fp32 (2^-24 of the mean, doubled for room)."""
+    HW = x.shape[2] * x.shape[3]
+    ref = x.mean((2, 3))
+    return ref, (HW + 4) * U53 * x.abs().mean((2, 3)) + 2 * U * ref.abs()
+
+
+def moments_ref(f: torch.Tensor, shift, s0: torch.Tensor, sxx0: torch.Tensor):
+    """(sum, bound, sxx, bound) of dp_feature_moments accumulating rows of f [rows, D] into s0 [D] / sxx0 [D, D], in float64.
+    d = f - shift is exact in fp64; each of the rows fp64 updates of an element rounds once (fma), so with the old value as one more
+    term the error is below (rows + 4) 2^-53 (sum_r |d_ri d_rj| + |old|)."""
+    d = f.double() - (shift.double() if shift is not None else 0.0)
+    rows = d.shape[0]
+    k = (rows + 4) * U53
+    return (s0 + d.sum(0), k * (d.abs().sum(0) + s0.abs()),
+            sxx0 + d.T @ d, k * (d.abs().T @ d.abs() + sxx0.abs()))
+
+
+def ddim_step_ref(x, e, nz, sb: float, sa: float, clip: float, sap: float, dirc: float, sigma: float):
+    """(ref, bound) of one DDIM update from the fp32 coefficients the scheduler passes: x0 = (x - sb e) / sa, clipped to +-clip when
+    clip > 0, out = sap x0 + dirc e (+ sigma noise).  x0 carries at most three roundings of |x| + sb |e| (product, difference,
+    division), 4 2^-24 (|x| + sb |e|) / sa, which sap scales; the clip is 1-Lipschitz, so a pre-clip x0 within that bound of +-clip
+    may land on either side; the update adds a few roundings of its terms."""
+    x, e = x.double(), e.double()
+    x0 = (x - sb * e) / sa
+    ex0 = 4 * U * (x.abs() + sb * e.abs()) / sa
+    if clip > 0:
+        x0 = x0.clamp(-clip, clip)
+    ref = sap * x0 + dirc * e
+    mag = sap * x0.abs() + dirc * e.abs()
+    if nz is not None and sigma != 0:
+        ref = ref + sigma * nz.double()
+        mag = mag + sigma * nz.double().abs()
+    return ref, sap * ex0 + 4 * U * mag
 
 
 def violations(got: torch.Tensor, ref: torch.Tensor, bound: torch.Tensor, limit: int = 8):

@@ -214,8 +214,13 @@ def _epilogue(lib, g, a, r, K, rows_out, ref, epi):
     return keep
 
 
-def replay_conv(lib, g, name, a, rep):
-    from diff_pruning_b200 import _lib as L
+DP_CONV_RELU = 4
+
+
+def replay_conv(lib, g, name, a, rep, chain=None):
+    """fprop / dgrad (fp32-grade) at the captured geometry.  With DP_CONV_RELU the fp64 reference takes the ReLU after every epilogue
+    term (1-Lipschitz: same bound).  chain(args, split-K workspace floats) -> (L, tensor-core launch?) overrides the box kernel's
+    chain length (the general-geometry and SIMT kernels of the evaluation census)."""
     N, H, W, Cin, P, Q, K, R, Sx = a.N, a.H, a.W, a.C, a.P, a.Q, a.K, a.R, a.S
     tc = bool(a.w_tc_hi)
     w, ck, kc, packs = _conv_weights(lib, g, K, Cin, R, Sx, tc)
@@ -259,6 +264,8 @@ def replay_conv(lib, g, name, a, rep):
     if acc:
         ref += init.double()
         epi += init.double().abs()
+    if a.flags & DP_CONV_RELU:
+        ref = ref.clamp_min(0.0)
     r.workspace = None
     ws, need = None, 0
     if a.workspace:
@@ -266,8 +273,11 @@ def replay_conv(lib, g, name, a, rep):
         if need > 0:
             ws = torch.full((need,), float("nan"), device="cuda")
             r.workspace = ws.data_ptr()
-    L_ = lc.chain_fprop(R * Sx, kg, lc.splitk_count(need, out.v.shape[0], out.v.shape[1], R * Sx * -(-kg // 64)))
-    assert not tc or L_ <= lc.L_MAX, f"{name}: chain of {L_} updates, beyond the {lc.L_MAX} at which the bound keeps its teeth"
+    if chain is not None:
+        L_, on_tc = chain(a, need)
+    else:
+        L_, on_tc = lc.chain_fprop(R * Sx, kg, lc.splitk_count(need, out.v.shape[0], out.v.shape[1], R * Sx * -(-kg // 64))), tc
+    assert not on_tc or L_ <= lc.L_MAX, f"{name}: chain of {L_} updates, beyond the {lc.L_MAX} at which the bound keeps its teeth"
     so = torch.zeros(1, dtype=torch.int32, device="cuda") if a.amax_out else None
     r.amax_out = so.data_ptr() if so is not None else None
 
