@@ -25,6 +25,9 @@ static inline int dp_check_launch() {
     if (!(cond)) return (code); \
   } while (0)
 
+// a nullable fp32 view [rows][ld] that float4 accesses may use: 16-byte aligned base, row pitch a multiple of 4
+static inline bool al16(const void* p, long long ld) { return p == nullptr || ((((uintptr_t)p) & 15) == 0 && (ld % 4) == 0); }
+
 static inline int ilog2_exact(int v) {  // log2 if power of two, else -1
   if (v <= 0 || (v & (v - 1))) return -1;
   int l = 0;

@@ -17,9 +17,9 @@
 // Both are instantiated per N tile width (64, 128, 192, 256): wgmma takes N as an immediate and the accumulators live in registers.
 #include <cuda.h>
 #include <cuda_bf16.h>
-#include <mutex>
 #include "common.cuh"
 #include "sm90.cuh"
+#include "sm90_host.cuh"
 
 namespace {
 using namespace sm90;
@@ -45,40 +45,6 @@ struct BfParams {
   int stages;
 };
 
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  uint32_t done;
-  do {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(done)
-        : "r"(bar), "r"(parity)
-        : "memory");
-  } while (!done);
-}
-__device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c0), "r"(c1), "r"(c2)
-      : "memory");
-}
 // ------------------------------------------------------------------------------------------------ fprop / dgrad
 // NB = N tile / 64 = rows of the weight box / 64
 template <int NB>
@@ -352,222 +318,171 @@ __global__ void pack_bf16_kernel(const float* __restrict__ w, int K, int C, int 
 }
 
 // ------------------------------------------------------------------------------------------------ host side
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-EncodeTiledFn g_encode = nullptr;
-int g_state = -1;
-int g_num_sms = 132;   // H100 SXM; bf_init reads the device's count
-std::mutex g_mutex;
-
 int bf_init() {
-  std::lock_guard<std::mutex> lk(g_mutex);
-  if (g_state >= 0) return g_state;
-  g_state = 0;
-  int dev = 0, major = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) { (void)cudaGetLastError(); return 0; }
-  if (cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev) != cudaSuccess || major != 9) { (void)cudaGetLastError(); return 0; }
-  void* fn = nullptr;
-  cudaDriverEntryPointQueryResult qres;
-  if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres) != cudaSuccess || !fn ||
-      qres != cudaDriverEntryPointSuccess) { (void)cudaGetLastError(); return 0; }
-  g_encode = (EncodeTiledFn)fn;
-  bool ok = true;
-  for (const void* k : {(const void*)conv_bf16_kernel<1>, (const void*)conv_bf16_kernel<2>, (const void*)conv_bf16_kernel<3>,
-                        (const void*)conv_bf16_kernel<4>, (const void*)wgrad_bf16_kernel<1>, (const void*)wgrad_bf16_kernel<2>,
-                        (const void*)wgrad_bf16_kernel<3>, (const void*)wgrad_bf16_kernel<4>})
-    ok = ok && cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, MAX_SMEM) == cudaSuccess;
-  cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev);
-  if (!ok) { (void)cudaGetLastError(); return 0; }
-  g_state = 1;
-  return 1;
-}
-
-bool make_map_bf16(CUtensorMap* m, const void* base, int rank, const cuuint64_t* dims, const cuuint64_t* strides_bytes,
-                   const cuuint32_t* box, int pix_stride = 1) {
-  cuuint32_t estr[5] = {1, (cuuint32_t)pix_stride, (cuuint32_t)pix_stride, 1, 1};
-  if (rank == 3) { estr[1] = 1; estr[2] = 1; }
-  return g_encode(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, (cuuint32_t)rank, const_cast<void*>(base), dims, strides_bytes, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-}
-
-// a box of `npix` pixels of an [N][H][W] grid as (bw, bh, bn) with bw*bh*bn == npix
-bool pick_box(int npix, int H, int W, int& bw, int& bh, int& bn) {
-  if (W >= npix) { if (W % npix) return false; bw = npix; bh = 1; bn = 1; return true; }
-  if (npix % W) return false;
-  bw = W;
-  int rem = npix / W;
-  if (H >= rem) { if (H % rem) return false; bh = rem; bn = 1; return true; }
-  if (rem % H) return false;
-  bh = H; bn = rem / H;
-  return true;
+  static const int ok = [] {
+    bool set = runtime().encode != nullptr;
+    for (const void* k : {(const void*)conv_bf16_kernel<1>, (const void*)conv_bf16_kernel<2>, (const void*)conv_bf16_kernel<3>,
+                          (const void*)conv_bf16_kernel<4>, (const void*)wgrad_bf16_kernel<1>, (const void*)wgrad_bf16_kernel<2>,
+                          (const void*)wgrad_bf16_kernel<3>, (const void*)wgrad_bf16_kernel<4>})
+      set = set && cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, MAX_SMEM) == cudaSuccess;
+    (void)cudaGetLastError();
+    return set ? 1 : 0;
+  }();
+  return ok;
 }
 
 int wrow_bf16(int c) { return (c + 63) & ~63; }
 
-struct TapTable { int n; signed char dh[9], dw[9], wt[9]; };
-
-TapTable dense_taps(int R, int S, int pad, bool flip) {
-  TapTable t{};
-  t.n = R * S;
-  for (int r = 0; r < R; ++r)
-    for (int s = 0; s < S; ++s) {
-      int i = r * S + s;
-      t.dh[i] = (signed char)(r - pad); t.dw[i] = (signed char)(s - pad);
-      t.wt[i] = (signed char)(flip ? (R * S - 1 - i) : i);
-    }
-  return t;
-}
-
-// act: bf16 [Nimg][H*in_stride][W*in_stride][ld_act] view with Kg valid channels; w: bf16 [T][Nout][wrow_bf16(Kg)]; out fp32 view.
-// dry = 1: only check eligibility.
-int launch_bf16(const void* act, long long ld_act, int Nimg, int H, int W, int Kg, const void* w, int Nout, int T, const TapTable& taps,
-                int os, int oa, int ob, int Ho, int Wo, float* out, long long ld_out, const float* bias, const float* rowadd,
-                long long ld_rowadd, const float* residual, long long ld_res, int accumulate, cudaStream_t st, int in_stride, int dry) {
+// Box, tiles, N tile and pipeline depth of one conv_bf16_kernel launch over an activation of pixel pitch ld_act (bf16 elements)
+struct BfPlan { int bw, bh, bn, tiles_m, n_tiles, bn_tile, stages; };
+int plan_bf16(const ConvGemm& g, long long ld_act, BfPlan& pl) {
   if (!bf_init()) return DP_ERR_UNSUPPORTED;
-  if (!dry && (!act || !w || !out)) return DP_ERR_NULL;
-  if (ld_act % 8 || ((uintptr_t)act & 15) || ((uintptr_t)w & 15) || Kg < 8 || Nout < 1) return DP_ERR_UNSUPPORTED;
-  int bw, bh, bn;
-  if (!pick_box(BM, H, W, bw, bh, bn)) return DP_ERR_UNSUPPORTED;
-  if (bw * in_stride > 256 || bh * in_stride > 256) return DP_ERR_UNSUPPORTED;
+  if (ld_act % 8 || g.Kg < 8 || g.Nout < 1 || !pick_box(BM, g.H, g.W, pl.bw, pl.bh, pl.bn)) return DP_ERR_UNSUPPORTED;
+  if (pl.bw * g.in_stride > 256 || pl.bh * g.in_stride > 256) return DP_ERR_UNSUPPORTED;
+  pl.tiles_m = (g.W / pl.bw) * (g.H / pl.bh) * ((g.N + pl.bn - 1) / pl.bn);
   // N tile: as wide as possible (<= 256) so the activation tile is fetched once; balanced over the tiles it takes, a multiple of 64
   // (one instantiation per width)
-  const int n_tiles = (Nout + 255) / 256;
-  int bn_tile = ((Nout + n_tiles - 1) / n_tiles + 63) & ~63;
-  if (bn_tile > 256) bn_tile = 256;
-  if (dry) return DP_OK;
+  pl.n_tiles = (g.Nout + 255) / 256;
+  pl.bn_tile = ((g.Nout + pl.n_tiles - 1) / pl.n_tiles + 63) & ~63;
+  if (pl.bn_tile > 256) pl.bn_tile = 256;
+  pl.stages = (MAX_SMEM - 2048) / (A_BYTES + pl.bn_tile * 128);     // every tile starts 1024-byte aligned
+  if (pl.stages > 8) pl.stages = 8;
+  return pl.stages < 2 ? DP_ERR_UNSUPPORTED : DP_OK;
+}
+
+// Operands and epilogue of a launch.  A: bf16 [N][H*in_stride][W*in_stride][ld_act] view of the GEMM's input; B: bf16 [T][Nout][wrow_bf16(Kg)];
+// out: fp32 [N][Ho][Wo][ld_out] view.
+struct BfLaunch {
+  const void* act; long long ld_act; const void* w; int T;
+  float* out; long long ld_out;
+  const float* bias; const float* rowadd; long long ld_rowadd; const float* residual; long long ld_res;
+  int accumulate;
+};
+// A convolution's launch: A = x (fprop) or dy (dgrad), B = its packed weights; the epilogue terms are fprop's
+BfLaunch conv_launch(const dp_conv_bf16_args* a, bool dgrad) {
+  BfLaunch l{};
+  l.act = dgrad ? a->dy_bf16 : a->x_bf16; l.ld_act = dgrad ? a->lddy : a->ldx; l.w = a->w_bf16; l.T = a->R * a->S;
+  l.out = a->out; l.ld_out = a->ld_out;
+  if (!dgrad) { l.bias = a->bias; l.rowadd = a->rowadd; l.ld_rowadd = a->ld_rowadd; l.residual = a->residual; l.ld_res = a->ld_res; }
+  l.accumulate = (a->flags & DP_CONV_ACCUMULATE) ? 1 : 0;
+  return l;
+}
+
+int launch_bf16(const ConvGemm& g, const BfLaunch& l, cudaStream_t st) {
+  if (!bf_init()) return DP_ERR_UNSUPPORTED;
+  if (!l.act || !l.w || !l.out) return DP_ERR_NULL;
+  if (((uintptr_t)l.act & 15) || ((uintptr_t)l.w & 15)) return DP_ERR_UNSUPPORTED;
+  BfPlan pl;
+  const int rc = plan_bf16(g, l.ld_act, pl);
+  if (rc != DP_OK) return rc;
   CUtensorMap mA, mB;
   {
-    const cuuint64_t Hin = (cuuint64_t)H * in_stride, Win = (cuuint64_t)W * in_stride;
-    cuuint64_t dims[4] = {(cuuint64_t)Kg, Win, Hin, (cuuint64_t)Nimg};
-    cuuint64_t str[3] = {(cuuint64_t)ld_act * 2, Win * ld_act * 2, Hin * Win * ld_act * 2};
-    cuuint32_t box[4] = {(cuuint32_t)KB, (cuuint32_t)(bw * in_stride), (cuuint32_t)(bh * in_stride), (cuuint32_t)bn};
-    if (!make_map_bf16(&mA, act, 4, dims, str, box, in_stride)) return DP_ERR_UNSUPPORTED;
+    const int s = g.in_stride;
+    const cuuint64_t Hin = (cuuint64_t)g.H * s, Win = (cuuint64_t)g.W * s;
+    cuuint64_t dims[4] = {(cuuint64_t)g.Kg, Win, Hin, (cuuint64_t)g.N};
+    cuuint64_t str[3] = {(cuuint64_t)l.ld_act * 2, Win * l.ld_act * 2, Hin * Win * l.ld_act * 2};
+    cuuint32_t box[4] = {(cuuint32_t)KB, (cuuint32_t)(pl.bw * s), (cuuint32_t)(pl.bh * s), (cuuint32_t)pl.bn};
+    if (!encode_map(&mA, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, l.act, 4, dims, str, box, s)) return DP_ERR_UNSUPPORTED;
   }
   {
-    const cuuint64_t ldb = (cuuint64_t)wrow_bf16(Kg);
-    cuuint64_t dims[3] = {ldb, (cuuint64_t)Nout, (cuuint64_t)T};
-    cuuint64_t str[2] = {ldb * 2, (cuuint64_t)Nout * ldb * 2};
-    cuuint32_t box[3] = {(cuuint32_t)KB, (cuuint32_t)bn_tile, 1};
-    if (!make_map_bf16(&mB, w, 3, dims, str, box)) return DP_ERR_UNSUPPORTED;
+    const cuuint64_t ldb = (cuuint64_t)wrow_bf16(g.Kg);
+    cuuint64_t dims[3] = {ldb, (cuuint64_t)g.Nout, (cuuint64_t)l.T};
+    cuuint64_t str[2] = {ldb * 2, (cuuint64_t)g.Nout * ldb * 2};
+    cuuint32_t box[3] = {(cuuint32_t)KB, (cuuint32_t)pl.bn_tile, 1};
+    if (!encode_map(&mB, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, l.w, 3, dims, str, box)) return DP_ERR_UNSUPPORTED;
   }
   BfParams p{};
-  p.Nimg = Nimg; p.Nout = Nout;
-  p.ntaps = taps.n;
-  for (int i = 0; i < 9; ++i) { p.dh[i] = taps.dh[i]; p.dw[i] = taps.dw[i]; p.wt[i] = taps.wt[i]; }
-  p.os = os; p.oa = oa; p.ob = ob; p.Ho = Ho; p.Wo = Wo; p.in_stride = in_stride;
-  p.kchunks = (Kg + KB - 1) / KB;
-  p.bw = bw; p.bh = bh; p.bn = bn; p.tiles_w = W / bw; p.tiles_h = H / bh;
-  p.y = out; p.ldy = ld_out; p.bias = bias; p.rowadd = rowadd; p.ld_rowadd = ld_rowadd; p.residual = residual; p.ld_res = ld_res;
-  p.accumulate = accumulate;
-  auto al16 = [](const void* q, long long ld) { return q == nullptr || ((((uintptr_t)q) & 15) == 0 && (ld % 4) == 0); };
-  p.vec4 = (al16(out, ld_out) && al16(bias, 0) && al16(rowadd, ld_rowadd) && al16(residual, ld_res)) ? 1 : 0;
-  const int stage_bytes = A_BYTES + bn_tile * 128;     // every tile starts 1024-byte aligned
-  int stages = (MAX_SMEM - 2048) / stage_bytes;
-  if (stages > 8) stages = 8;
-  if (stages < 2) return DP_ERR_UNSUPPORTED;
-  p.stages = stages;
-  const int tiles_n = (Nimg + bn - 1) / bn;
-  const int tiles_m = p.tiles_w * p.tiles_h * tiles_n, total = tiles_m * n_tiles;
-  const int ctas = total < g_num_sms ? total : g_num_sms;
-  const size_t smem = (size_t)stages * stage_bytes + 2048;
-  switch (bn_tile / 64) {
-    case 1: conv_bf16_kernel<1><<<ctas, THREADS, smem, st>>>(mA, mB, p, tiles_m, total); break;
-    case 2: conv_bf16_kernel<2><<<ctas, THREADS, smem, st>>>(mA, mB, p, tiles_m, total); break;
-    case 3: conv_bf16_kernel<3><<<ctas, THREADS, smem, st>>>(mA, mB, p, tiles_m, total); break;
-    default: conv_bf16_kernel<4><<<ctas, THREADS, smem, st>>>(mA, mB, p, tiles_m, total); break;
+  p.Nimg = g.N; p.Nout = g.Nout;
+  p.ntaps = g.taps.n;
+  for (int i = 0; i < 9; ++i) { p.dh[i] = g.taps.dh[i]; p.dw[i] = g.taps.dw[i]; p.wt[i] = g.taps.wt[i]; }
+  p.os = g.os; p.oa = g.oa; p.ob = g.ob; p.Ho = g.Ho; p.Wo = g.Wo; p.in_stride = g.in_stride;
+  p.kchunks = (g.Kg + KB - 1) / KB;
+  p.bw = pl.bw; p.bh = pl.bh; p.bn = pl.bn; p.tiles_w = g.W / pl.bw; p.tiles_h = g.H / pl.bh;
+  p.y = l.out; p.ldy = l.ld_out; p.bias = l.bias; p.rowadd = l.rowadd; p.ld_rowadd = l.ld_rowadd; p.residual = l.residual; p.ld_res = l.ld_res;
+  p.accumulate = l.accumulate;
+  p.vec4 = (al16(l.out, l.ld_out) && al16(l.bias, 0) && al16(l.rowadd, l.ld_rowadd) && al16(l.residual, l.ld_res)) ? 1 : 0;
+  p.stages = pl.stages;
+  const int total = pl.tiles_m * pl.n_tiles, sms = runtime().num_sms, ctas = total < sms ? total : sms;
+  const size_t smem = (size_t)pl.stages * (A_BYTES + pl.bn_tile * 128) + 2048;
+  switch (pl.bn_tile / 64) {
+    case 1: conv_bf16_kernel<1><<<ctas, THREADS, smem, st>>>(mA, mB, p, pl.tiles_m, total); break;
+    case 2: conv_bf16_kernel<2><<<ctas, THREADS, smem, st>>>(mA, mB, p, pl.tiles_m, total); break;
+    case 3: conv_bf16_kernel<3><<<ctas, THREADS, smem, st>>>(mA, mB, p, pl.tiles_m, total); break;
+    default: conv_bf16_kernel<4><<<ctas, THREADS, smem, st>>>(mA, mB, p, pl.tiles_m, total); break;
   }
   return dp_check_launch();
 }
 
 bool conv_shape_ok(const dp_conv_bf16_args* a) {
-  if (!a) return false;
-  if (a->R != a->S || (a->R != 1 && a->R != 3) || a->pad_l != a->pad_t) return false;
-  if (!((a->stride == 1 && a->pad_t == (a->R - 1) / 2) || (a->stride == 2 && a->R == 3 && (a->pad_t == 0 || a->pad_t == 1)))) return false;
-  if (a->P * a->stride != a->H || a->Q * a->stride != a->W) return false;
-  if (a->N <= 0 || a->H <= 0 || a->W <= 0 || a->C <= 0 || a->K <= 0) return false;
-  return true;
+  return a && box_geometry(a) && a->N > 0 && a->H > 0 && a->W > 0 && a->C > 0 && a->K > 0;
 }
 
-int fprop_impl(const dp_conv_bf16_args* a, cudaStream_t st, int dry) {
-  if (!conv_shape_ok(a) || a->ldx < a->C || a->ld_out < a->K) return DP_ERR_UNSUPPORTED;
-  return launch_bf16(a->x_bf16, a->ldx, a->N, a->P, a->Q, a->C, a->w_bf16, a->K, a->R * a->S, dense_taps(a->R, a->S, a->pad_t, false), 1, 0, 0,
-                     a->P, a->Q, a->out, a->ld_out, a->bias, a->rowadd, a->ld_rowadd, a->residual, a->ld_res,
-                     (a->flags & DP_CONV_ACCUMULATE) ? 1 : 0, st, a->stride, dry);
+// The GEMMs of a fprop (op 0) or dgrad (op 1), or 0 when the bf16 kernels do not take the convolution's geometry
+int bf16_gemms(const dp_conv_bf16_args* a, int op, ConvGemm g[4]) {
+  if (!conv_shape_ok(a)) return 0;
+  if (op == 0 ? (a->ldx < a->C || a->ld_out < a->K) : (a->lddy < a->K || a->ld_out < a->C)) return 0;
+  return conv_gemms(a, op, g);
 }
 
-int dgrad_impl(const dp_conv_bf16_args* a, cudaStream_t st, int dry) {
-  if (!conv_shape_ok(a) || a->lddy < a->K || a->ld_out < a->C) return DP_ERR_UNSUPPORTED;
-  const int acc = (a->flags & DP_CONV_ACCUMULATE) ? 1 : 0;
-  if (a->stride == 1)
-    return launch_bf16(a->dy_bf16, a->lddy, a->N, a->H, a->W, a->K, a->w_bf16, a->C, a->R * a->S, dense_taps(a->R, a->S, a->pad_t, true), 1, 0, 0,
-                       a->H, a->W, a->out, a->ld_out, nullptr, nullptr, 0, nullptr, 0, acc, st, 1, dry);
-  // stride 2: dx[2i+a, 2j+b] only sees taps with (a+pad-r), (b+pad-s) even -> 4 parity classes, each a dense GEMM over the dy grid
-  TapTable cls[4];
-  for (int ca = 0; ca < 2; ++ca)
-    for (int cb = 0; cb < 2; ++cb) {
-      TapTable& t = cls[ca * 2 + cb];
-      t = TapTable{};
-      for (int r = 0; r < 3; ++r)
-        for (int s = 0; s < 3; ++s) {
-          int nh = ca + a->pad_t - r, nw = cb + a->pad_l - s;
-          if ((nh & 1) || (nw & 1)) continue;
-          t.dh[t.n] = (signed char)(nh / 2); t.dw[t.n] = (signed char)(nw / 2); t.wt[t.n] = (signed char)(r * 3 + s);
-          ++t.n;
-        }
-      if (t.n == 0) return DP_ERR_UNSUPPORTED;
-    }
-  for (int ca = 0; ca < 2; ++ca)
-    for (int cb = 0; cb < 2; ++cb) {
-      int rc = launch_bf16(a->dy_bf16, a->lddy, a->N, a->P, a->Q, a->K, a->w_bf16, a->C, 9, cls[ca * 2 + cb], 2, ca, cb, a->H, a->W, a->out,
-                           a->ld_out, nullptr, nullptr, 0, nullptr, 0, acc, st, 1, dry);
-      if (rc != DP_OK) return rc;
-      if (dry) break;
-    }
+int conv_bf16(const dp_conv_bf16_args* a, int op, cudaStream_t st) {
+  ConvGemm g[4];
+  const int n = bf16_gemms(a, op, g);
+  if (n == 0) return DP_ERR_UNSUPPORTED;
+  const BfLaunch l = conv_launch(a, op != 0);
+  for (int c = 0; c < n; ++c) {
+    const int rc = launch_bf16(g[c], l, st);
+    if (rc != DP_OK) return rc;
+  }
   return DP_OK;
 }
 
-int wgrad_impl(const dp_conv_bf16_args* a, cudaStream_t st, int dry) {
-  if (!conv_shape_ok(a) || a->splits < 1 || a->ldx < a->C || a->lddy < a->K) return DP_ERR_UNSUPPORTED;
-  if (!bf_init()) return DP_ERR_UNSUPPORTED;
-  if (!dry && (!a->x_bf16 || !a->dy_bf16 || !a->workspace)) return DP_ERR_NULL;
-  if (a->ldx % 8 || a->lddy % 8 || ((uintptr_t)a->x_bf16 & 15) || ((uintptr_t)a->dy_bf16 & 15)) return DP_ERR_UNSUPPORTED;
-  int bw, bh, bn;
-  if (!pick_box(WG_PIX, a->P, a->Q, bw, bh, bn)) return DP_ERR_UNSUPPORTED;   // 64-pixel chunks of the dy grid
-  if (a->N % bn) return DP_ERR_UNSUPPORTED;
-  if (bw * a->stride > 256 || bh * a->stride > 256) return DP_ERR_UNSUPPORTED;
-  if (dry) return DP_OK;
+bool wgrad_geometry(const dp_conv_bf16_args* a) { return conv_shape_ok(a) && a->splits >= 1 && a->ldx >= a->C && a->lddy >= a->K; }
+
+// Box (64 pixels of the dy grid), in-channel tile and pipeline depth of a wgrad_bf16_kernel launch
+struct WgBfPlan { int bw, bh, bn, ct_width, stages; };
+int plan_wgrad_bf16(const dp_conv_bf16_args* a, WgBfPlan& pl) {
+  if (!bf_init() || a->ldx % 8 || a->lddy % 8) return DP_ERR_UNSUPPORTED;
+  if (!pick_box(WG_PIX, a->P, a->Q, pl.bw, pl.bh, pl.bn) || a->N % pl.bn) return DP_ERR_UNSUPPORTED;
+  if (pl.bw * a->stride > 256 || pl.bh * a->stride > 256) return DP_ERR_UNSUPPORTED;
+  pl.ct_width = dp_bf16_wgrad_ctile(a->C);
+  pl.stages = (MAX_SMEM - 2048) / ((2 + pl.ct_width / 64) * BLK_BYTES);
+  if (pl.stages > 8) pl.stages = 8;
+  return DP_OK;
+}
+
+int wgrad_bf16(const dp_conv_bf16_args* a, cudaStream_t st) {
+  if (!wgrad_geometry(a) || !bf_init()) return DP_ERR_UNSUPPORTED;
+  if (!a->x_bf16 || !a->dy_bf16 || !a->workspace) return DP_ERR_NULL;
+  if (((uintptr_t)a->x_bf16 & 15) || ((uintptr_t)a->dy_bf16 & 15)) return DP_ERR_UNSUPPORTED;
+  WgBfPlan pl;
+  const int rc = plan_wgrad_bf16(a, pl);
+  if (rc != DP_OK) return rc;
   CUtensorMap mDy, mX;
   {
     cuuint64_t dims[4] = {(cuuint64_t)a->K, (cuuint64_t)a->Q, (cuuint64_t)a->P, (cuuint64_t)a->N};
     cuuint64_t str[3] = {(cuuint64_t)a->lddy * 2, (cuuint64_t)a->Q * a->lddy * 2, (cuuint64_t)a->P * a->Q * a->lddy * 2};
-    cuuint32_t box[4] = {64, (cuuint32_t)bw, (cuuint32_t)bh, (cuuint32_t)bn};
-    if (!make_map_bf16(&mDy, a->dy_bf16, 4, dims, str, box)) return DP_ERR_UNSUPPORTED;
+    cuuint32_t box[4] = {64, (cuuint32_t)pl.bw, (cuuint32_t)pl.bh, (cuuint32_t)pl.bn};
+    if (!encode_map(&mDy, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, a->dy_bf16, 4, dims, str, box)) return DP_ERR_UNSUPPORTED;
   }
   {
     cuuint64_t dims[4] = {(cuuint64_t)a->C, (cuuint64_t)a->W, (cuuint64_t)a->H, (cuuint64_t)a->N};
     cuuint64_t str[3] = {(cuuint64_t)a->ldx * 2, (cuuint64_t)a->W * a->ldx * 2, (cuuint64_t)a->H * a->W * a->ldx * 2};
-    cuuint32_t box[4] = {64, (cuuint32_t)(bw * a->stride), (cuuint32_t)(bh * a->stride), (cuuint32_t)bn};
-    if (!make_map_bf16(&mX, a->x_bf16, 4, dims, str, box, a->stride)) return DP_ERR_UNSUPPORTED;
+    cuuint32_t box[4] = {64, (cuuint32_t)(pl.bw * a->stride), (cuuint32_t)(pl.bh * a->stride), (cuuint32_t)pl.bn};
+    if (!encode_map(&mX, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, a->x_bf16, 4, dims, str, box, a->stride)) return DP_ERR_UNSUPPORTED;
   }
   WgBfParams p{};
   p.Nimg = a->N; p.H = a->P; p.W = a->Q; p.C = a->C; p.K = a->K; p.R = a->R; p.S = a->S; p.pad = a->pad_t; p.in_stride = a->stride;
-  p.bw = bw; p.bh = bh; p.bn = bn; p.tiles_w = a->Q / bw; p.tiles_h = a->P / bh;
-  p.total_chunks = p.tiles_w * p.tiles_h * (a->N / bn);
+  p.bw = pl.bw; p.bh = pl.bh; p.bn = pl.bn; p.tiles_w = a->Q / pl.bw; p.tiles_h = a->P / pl.bh;
+  p.total_chunks = p.tiles_w * p.tiles_h * (a->N / pl.bn);
   p.chunks_per_split = (p.total_chunks + a->splits - 1) / a->splits;
-  p.ct_width = dp_bf16_wgrad_ctile(a->C);
+  p.ct_width = pl.ct_width;
   p.c_tiles = (a->C + p.ct_width - 1) / p.ct_width;
-  const int x_blocks = p.ct_width / 64;
   p.ws = a->workspace;
-  const int stage_bytes = (2 + x_blocks) * BLK_BYTES;
-  int stages = (MAX_SMEM - 2048) / stage_bytes;
-  if (stages > 8) stages = 8;
-  p.stages = stages;
+  p.stages = pl.stages;
   const int k_tiles = (a->K + 127) / 128;
   dim3 grid((unsigned)(k_tiles * p.c_tiles * a->R * a->S), (unsigned)a->splits);
-  const size_t smem = (size_t)stages * stage_bytes + 2048;
-  switch (x_blocks) {
+  const size_t smem = (size_t)pl.stages * (2 + pl.ct_width / 64) * BLK_BYTES + 2048;
+  switch (pl.ct_width / 64) {
     case 1: wgrad_bf16_kernel<1><<<grid, THREADS, smem, st>>>(mDy, mX, p); break;
     case 2: wgrad_bf16_kernel<2><<<grid, THREADS, smem, st>>>(mDy, mX, p); break;
     case 3: wgrad_bf16_kernel<3><<<grid, THREADS, smem, st>>>(mDy, mX, p); break;
@@ -588,15 +503,20 @@ extern "C" int dp_bf16_wgrad_ctile(int C) {
   return w > 256 ? 256 : w;
 }
 
-extern "C" int dp_conv2d_fprop_bf16(const dp_conv_bf16_args* a, dp_stream_t s) { return fprop_impl(a, (cudaStream_t)s, 0); }
-extern "C" int dp_conv2d_dgrad_bf16(const dp_conv_bf16_args* a, dp_stream_t s) { return dgrad_impl(a, (cudaStream_t)s, 0); }
-extern "C" int dp_conv2d_wgrad_bf16(const dp_conv_bf16_args* a, dp_stream_t s) { return wgrad_impl(a, (cudaStream_t)s, 0); }
+extern "C" int dp_conv2d_fprop_bf16(const dp_conv_bf16_args* a, dp_stream_t s) { return conv_bf16(a, 0, (cudaStream_t)s); }
+extern "C" int dp_conv2d_dgrad_bf16(const dp_conv_bf16_args* a, dp_stream_t s) { return conv_bf16(a, 1, (cudaStream_t)s); }
+extern "C" int dp_conv2d_wgrad_bf16(const dp_conv_bf16_args* a, dp_stream_t s) { return wgrad_bf16(a, (cudaStream_t)s); }
 // op: 0 fprop, 1 dgrad, 2 wgrad.  DP_OK when the bf16 kernels take this shape (pointers are not needed), else DP_ERR_UNSUPPORTED.
 extern "C" int dp_conv_bf16_eligible(const dp_conv_bf16_args* a, int op) {
   if (!a) return DP_ERR_NULL;
-  dp_conv_bf16_args b = *a;     // alignment checks see aligned dummies
-  b.x_bf16 = b.dy_bf16 = b.w_bf16 = nullptr;
-  return op == 0 ? fprop_impl(&b, nullptr, 1) : op == 1 ? dgrad_impl(&b, nullptr, 1) : wgrad_impl(&b, nullptr, 1);
+  if (op != 0 && op != 1) {
+    WgBfPlan pl;
+    return wgrad_geometry(a) ? plan_wgrad_bf16(a, pl) : DP_ERR_UNSUPPORTED;
+  }
+  ConvGemm g[4];
+  BfPlan pl;
+  // the parity classes of a stride-2 dgrad share their grid and channels: the first stands for all four
+  return bf16_gemms(a, op, g) ? plan_bf16(g[0], op == 0 ? a->ldx : a->lddy, pl) : DP_ERR_UNSUPPORTED;
 }
 
 extern "C" int dp_cvt_bf16(const float* src, int64_t ld, int64_t rows, int32_t C, void* dst, int64_t ld_dst, dp_stream_t stream) {
@@ -606,7 +526,7 @@ extern "C" int dp_cvt_bf16(const float* src, int64_t ld, int64_t rows, int32_t C
   const int vec_ok = (((uintptr_t)src & 15) == 0 && ld % 4 == 0) ? 1 : 0;
   const long long total = rows * (ld_dst / 8);
   long long blocks = (total + 255) / 256;
-  if (blocks > g_num_sms * 32) blocks = g_num_sms * 32;
+  if (blocks > runtime().num_sms * 32) blocks = runtime().num_sms * 32;
   cvt_bf16_kernel<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(src, ld, rows, C, (__nv_bfloat16*)dst, ld_dst, vec_ok);
   return dp_check_launch();
 }
@@ -617,7 +537,7 @@ extern "C" int dp_pack_conv_weight_bf16(const float* w, int32_t K, int32_t C, in
   const int Cp = wrow_bf16(C), Kp = wrow_bf16(K);
   long long total = (long long)R * S * ((long long)K * Cp > (long long)C * Kp ? (long long)K * Cp : (long long)C * Kp);
   int blocks = (int)((total + 255) / 256);
-  if (blocks > g_num_sms * 16) blocks = g_num_sms * 16;
+  if (blocks > runtime().num_sms * 16) blocks = runtime().num_sms * 16;
   pack_bf16_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(w, K, C, R * S, Cp, Kp, (__nv_bfloat16*)kc, (__nv_bfloat16*)ck);
   return dp_check_launch();
 }

@@ -23,9 +23,9 @@
 //   pack / split / transpose helpers; dp_gemm_nt_tc runs the attention GEMMs on the persistent kernel.
 #include <cuda.h>
 #include <cuda_fp16.h>
-#include <mutex>
 #include "common.cuh"
 #include "sm90.cuh"
+#include "sm90_host.cuh"
 
 namespace {
 using namespace sm90;
@@ -68,47 +68,6 @@ struct TcParams {
   int relu;
 };
 
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  uint32_t done;
-  do {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(done)
-        : "r"(bar), "r"(parity)
-        : "memory");
-  } while (!done);
-}
-__device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-// 16-byte cp.async with zero fill past src_bytes (0 = nothing read), and the mbarrier arrival that fires when this thread's copies land
-__device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, uint32_t src_bytes) {
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(src_bytes) : "memory");
-}
-__device__ __forceinline__ void cp_async_mbar_arrive(uint32_t bar) {
-  asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c0), "r"(c1), "r"(c2)
-      : "memory");
-}
 // amax slot -> power-of-two scale.  E = biased exponent of the bound (|v| < 2^(E-126)), clamped so that both factors are normal floats;
 // up = 2^(140-E) brings the operand below 2^14 (fp16 overflows at 65504), dn = 2^(E-140) undoes it in the epilogue.
 __device__ __forceinline__ int amax_exponent(const uint32_t* slot) {
@@ -624,13 +583,6 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap mapDy, const __grid_constant
 }
 
 // ------------------------------------------------------------------------------------------------ host side
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-EncodeTiledFn g_encode = nullptr;
-int g_tc_state = -1;  // -1 unknown, 0 unavailable, 1 ok
-int g_num_sms = 132;   // H100 SXM; tc_init reads the device's count
-std::mutex g_tc_mutex;
 constexpr int PS_SMEM = PS_STAGES * PS_STAGE_BYTES + 2048;
 constexpr int WG_SMEM = WG_STAGES * WG_STAGE_BYTES + 2048;
 
@@ -640,64 +592,24 @@ constexpr int WG_SMEM = WG_STAGES * WG_STAGE_BYTES + 2048;
 static int wrow(int c) { return c > 64 ? ((c + 63) & ~63) : ((c + 7) & ~7); }
 
 int tc_init() {
-  std::lock_guard<std::mutex> lk(g_tc_mutex);
-  if (g_tc_state >= 0) return g_tc_state;
-  g_tc_state = 0;
-  int dev = 0, major = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) { (void)cudaGetLastError(); return 0; }
-  if (cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev) != cudaSuccess || major != 9) { (void)cudaGetLastError(); return 0; }
-  void* fn = nullptr;
-  cudaDriverEntryPointQueryResult qres;
-  if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres) != cudaSuccess || !fn ||
-      qres != cudaDriverEntryPointSuccess) { (void)cudaGetLastError(); return 0; }
-  g_encode = (EncodeTiledFn)fn;
-  bool ok = cudaFuncSetAttribute(conv_tc_ps_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, PS_SMEM) == cudaSuccess;
-  ok = ok && cudaFuncSetAttribute(conv_tc_ps_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, PS_SMEM) == cudaSuccess;
-  ok = ok && cudaFuncSetAttribute(wgrad_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_SMEM) == cudaSuccess;
-  cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev);
-  if (!ok) { (void)cudaGetLastError(); return 0; }
-  (void)cudaGetLastError();
-  g_tc_state = 1;
-  return 1;
+  static const int ok = [] {
+    const bool set = runtime().encode &&
+        cudaFuncSetAttribute(conv_tc_ps_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, PS_SMEM) == cudaSuccess &&
+        cudaFuncSetAttribute(conv_tc_ps_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, PS_SMEM) == cudaSuccess &&
+        cudaFuncSetAttribute(wgrad_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_SMEM) == cudaSuccess;
+    (void)cudaGetLastError();
+    return set ? 1 : 0;
+  }();
+  return ok;
 }
 
-// pix_stride > 1 (strided convolution): dims 1 and 2 (W, H) are traversed with that element stride; the caller passes the box
-// extents in traversed elements (box = loaded pixels x pix_stride)
-bool make_map(CUtensorMap* m, const void* base, int rank, const cuuint64_t* dims, const cuuint64_t* strides_bytes,
-              const cuuint32_t* box, CUtensorMapSwizzle swz = CU_TENSOR_MAP_SWIZZLE_128B, int pix_stride = 1,
-              CUtensorMapDataType dtype = CU_TENSOR_MAP_DATA_TYPE_FLOAT32) {
-  cuuint32_t estr[5] = {1, (cuuint32_t)pix_stride, (cuuint32_t)pix_stride, 1, 1};
-  CUresult r = g_encode(m, dtype, (cuuint32_t)rank, const_cast<void*>(base), dims, strides_bytes, box, estr,
-                        CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  return r == CUDA_SUCCESS;
-}
-
-// 128-pixel box of an [N][H][W] grid
-bool pick_box(int N, int H, int W, int& bw, int& bh, int& bn) {
-  if (W >= BM) {
-    if (W % BM) return false;
-    bw = BM; bh = 1; bn = 1; return true;
-  }
-  if (BM % W) return false;
-  bw = W;
-  int rem = BM / W;
-  if (H >= rem) {
-    if (H % rem) return false;
-    bh = rem; bn = 1; return true;
-  }
-  if (rem % H) return false;
-  bh = H; bn = rem / H;
-  return true;
-}
-
-struct TapTable { int n; signed char dh[9], dw[9], wt[9]; };
 // K splits of a persistent-kernel launch with `tiles` output tiles of `iters` pipeline stages each: enough work items to fill the SMs,
 // at least 4 stages per split, none when the tiles already cover half the machine
 static int pick_ksplit(int tiles, int iters, int& it_per_split) {
   it_per_split = iters;
-  if (tiles * 2 > g_num_sms || iters < 8) return 1;
-  int ks = g_num_sms / tiles;
+  const int sms = runtime().num_sms;
+  if (tiles * 2 > sms || iters < 8) return 1;
+  int ks = sms / tiles;
   if (ks > iters / 4) ks = iters / 4;
   if (ks > 16) ks = 16;
   if (ks < 2) return 1;
@@ -705,83 +617,109 @@ static int pick_ksplit(int tiles, int iters, int& it_per_split) {
   return (iters + it_per_split - 1) / it_per_split;      // no empty split
 }
 
-// Shared launcher.  act: [Nimg][H][W][Kg] fp32 view (ld_act) = A operand on whose pixel grid the M tiles live, amax_a its amax slot;
-// w_hi / w_lo: fp16 [T][Nout][ldb] with the scale of slot amax_b; out: [Nimg][Ho][Wo][Nout] view, output pixel = (p*os+oa, q*os+ob).
-// ws: optional split-K workspace (dp_conv_splitk_workspace_floats floats); *ws_need != nullptr: only report the floats a split launch needs
-int launch_tc(const float* act, long long ld_act, const uint32_t* amax_a, int Nimg, int H, int W, int Kg, const void* w_hi, const void* w_lo,
-              const uint32_t* amax_b, int Nout, int T, const TapTable& taps, int os, int oa, int ob, int Ho, int Wo, float* out,
-              long long ld_out, const float* bias, const float* rowadd, long long ld_rowadd, const float* residual, long long ld_res,
-              int accumulate, cudaStream_t st, float alpha = 1.0f, int b_from_img = 0, int in_stride = 1, int ldb = -1, float* ws = nullptr,
-              long long* ws_need = nullptr, uint32_t* amax_out = nullptr) {
-  if (ldb < 0) ldb = wrow(Kg);   // packed conv weights; batched GEMM callers pass their own row pitch
+// Tiles and K split of one conv_tc_ps_kernel launch.  M tiles: 128-pixel boxes of the GEMM's grid, or with `flat` (the general-geometry
+// kernel) 128 consecutive pixels of its [1][1][M] grid; N tiles of 128 channels.  With `split` (the launch has a workspace) a launch too
+// small to fill the SMs splits its K loop; ws_floats is the workspace that takes.
+struct TcPlan { int bw, bh, bn, tiles_w, tiles_h, tiles_m, n_tiles, ksplit, it_per_split; long long ws_floats; };
+int plan_tc(const ConvGemm& g, bool flat, bool split, TcPlan& pl) {
   if (!tc_init()) return DP_ERR_UNSUPPORTED;
-  if (!ws_need && (!w_hi || !w_lo || !amax_a || !amax_b)) return DP_ERR_UNSUPPORTED;
-  if (!ws_need && (ld_act % 4 || ((uintptr_t)act & 15) || ((uintptr_t)w_hi & 15) || ((uintptr_t)w_lo & 15))) return DP_ERR_UNSUPPORTED;
-  int bw, bh, bn;
-  if (!pick_box(Nimg, H, W, bw, bh, bn)) return DP_ERR_UNSUPPORTED;
-  constexpr int BN = 128;
-  if (ws_need) {     // geometry-only query
-    *ws_need = 0;
-    if (b_from_img) return DP_OK;
-    const int tiles_m = (W / bw) * (H / bh) * ((Nimg + bn - 1) / bn), n_tiles = (Nout + 127) / 128;
-    int ips;
-    const int ks = pick_ksplit(tiles_m * n_tiles, taps.n * ((Kg + BK - 1) / BK), ips);
-    if (ks > 1) *ws_need = (long long)ks * tiles_m * BM * n_tiles * 128;
-    return DP_OK;
-  }
-  if (b_from_img && bn != 1) return DP_ERR_UNSUPPORTED;
+  if (flat) { pl.bw = BM; pl.bh = 1; pl.bn = 1; }
+  else if (!pick_box(BM, g.H, g.W, pl.bw, pl.bh, pl.bn)) return DP_ERR_UNSUPPORTED;
+  pl.tiles_w = (g.W + pl.bw - 1) / pl.bw; pl.tiles_h = g.H / pl.bh;
+  pl.tiles_m = pl.tiles_w * pl.tiles_h * ((g.N + pl.bn - 1) / pl.bn);
+  pl.n_tiles = (g.Nout + PS_BN - 1) / PS_BN;
+  const int iters = g.taps.n * ((g.Kg + BK - 1) / BK);
+  pl.ksplit = 1; pl.it_per_split = iters;
+  if (split) pl.ksplit = pick_ksplit(pl.tiles_m * pl.n_tiles, iters, pl.it_per_split);
+  pl.ws_floats = pl.ksplit > 1 ? (long long)pl.ksplit * pl.tiles_m * BM * pl.n_tiles * PS_BN : 0;
+  return DP_OK;
+}
+
+// Operands and epilogue of a launch.  A: fp32 NHWC view [N][H*in_stride][W*in_stride][ld_act] of the GEMM's input with amax slot amax_a;
+// B: fp16 hi / lo' [T][Nout][ldb] with the scale of slot amax_b (ldb -1: packed conv weights, wrow(Kg)); out: [N][Ho][Wo][ld_out] view.
+// ws: optional split-K workspace (dp_conv_splitk_workspace_floats floats).
+struct TcLaunch {
+  const float* act; long long ld_act; const uint32_t* amax_a;
+  const void* w_hi; const void* w_lo; const uint32_t* amax_b; int T; int ldb = -1;
+  float* out; long long ld_out;
+  const float* bias = nullptr; const float* rowadd = nullptr; long long ld_rowadd = 0; const float* residual = nullptr; long long ld_res = 0;
+  int accumulate = 0;
+  float* ws = nullptr;
+  uint32_t* amax_out = nullptr;
+  float alpha = 1.0f;                      // epilogue scale of the accumulator (attention logits)
+  int b_from_img = 0;                      // batched GEMM: B "tap" = the tile's image
+  const dp_conv_args* gather = nullptr;    // general-geometry fprop of this convolution: the kernel gathers A from x itself
+};
+
+// A convolution's launch: A = x (fprop) or dy (dgrad), B = its packed weights, out = y or dx; the epilogue terms are fprop's
+TcLaunch conv_launch(const dp_conv_args* a, bool dgrad) {
+  TcLaunch l{};
+  l.act = (const float*)(dgrad ? a->y : a->x); l.ld_act = dgrad ? a->ldy : a->ldx; l.amax_a = dgrad ? a->amax_y : a->amax_x;
+  l.w_hi = a->w_tc_hi; l.w_lo = a->w_tc_lo; l.amax_b = a->amax_w; l.T = a->R * a->S;
+  l.out = (float*)(dgrad ? a->x : a->y); l.ld_out = dgrad ? a->ldx : a->ldy;
+  if (!dgrad) { l.bias = a->bias; l.rowadd = a->rowadd; l.ld_rowadd = a->ld_rowadd; l.residual = a->residual; l.ld_res = a->ld_res; }
+  l.accumulate = (a->flags & DP_CONV_ACCUMULATE) ? 1 : 0;
+  l.ws = a->workspace; l.amax_out = a->amax_out;
+  return l;
+}
+
+int launch_tc(const ConvGemm& g, const TcLaunch& l, cudaStream_t st) {
+  const bool any = l.gather != nullptr, split = l.ws && !l.b_from_img;
+  TcPlan pl;
+  if (plan_tc(g, any, split, pl) != DP_OK) return DP_ERR_UNSUPPORTED;
+  if (!l.w_hi || !l.w_lo || !l.amax_a || !l.amax_b) return DP_ERR_UNSUPPORTED;
+  if (l.ld_act % 4 || ((uintptr_t)l.act & 15) || ((uintptr_t)l.w_hi & 15) || ((uintptr_t)l.w_lo & 15)) return DP_ERR_UNSUPPORTED;
+  if (l.b_from_img && pl.bn != 1) return DP_ERR_UNSUPPORTED;
   CUtensorMap mA, mBh, mBl;
-  {
+  if (!any) {
     // strided fprop: the M tiles live on the OUTPUT grid [H][W]; the activation is [H*in_stride][W*in_stride] and the box picks every
     // in_stride-th pixel (TMA element strides), so a tile is still one 128-pixel box
-    const cuuint64_t Hin = (cuuint64_t)H * in_stride, Win = (cuuint64_t)W * in_stride;
-    cuuint64_t dims[4] = {(cuuint64_t)Kg, Win, Hin, (cuuint64_t)Nimg};
-    cuuint64_t str[3] = {(cuuint64_t)ld_act * 4, Win * ld_act * 4, Hin * Win * ld_act * 4};
-    cuuint32_t box[4] = {32u, (cuuint32_t)(bw * in_stride), (cuuint32_t)(bh * in_stride), (cuuint32_t)bn};   // two boxes of 32 fp32 channels per stage
+    const int s = g.in_stride;
+    const cuuint64_t Hin = (cuuint64_t)g.H * s, Win = (cuuint64_t)g.W * s;
+    cuuint64_t dims[4] = {(cuuint64_t)g.Kg, Win, Hin, (cuuint64_t)g.N};
+    cuuint64_t str[3] = {(cuuint64_t)l.ld_act * 4, Win * l.ld_act * 4, Hin * Win * l.ld_act * 4};
+    cuuint32_t box[4] = {32u, (cuuint32_t)(pl.bw * s), (cuuint32_t)(pl.bh * s), (cuuint32_t)pl.bn};   // two boxes of 32 fp32 channels per stage
     if (box[1] > 256 || box[2] > 256) return DP_ERR_UNSUPPORTED;
-    if (!make_map(&mA, act, 4, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B, in_stride)) return DP_ERR_UNSUPPORTED;
+    if (!encode_map(&mA, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, l.act, 4, dims, str, box, s)) return DP_ERR_UNSUPPORTED;
   }
   {
-    const cuuint64_t Kp = (cuuint64_t)ldb;
+    const cuuint64_t Kp = (cuuint64_t)(l.ldb < 0 ? wrow(g.Kg) : l.ldb);
     if (Kp % 8) return DP_ERR_UNSUPPORTED;
-    cuuint64_t dims[3] = {Kp, (cuuint64_t)Nout, (cuuint64_t)T};
-    cuuint64_t str[2] = {Kp * 2, (cuuint64_t)Nout * Kp * 2};
-    cuuint32_t box[3] = {(cuuint32_t)BK, (cuuint32_t)BN, 1};
-    if (!make_map(&mBh, w_hi, 3, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B, 1, CU_TENSOR_MAP_DATA_TYPE_FLOAT16) ||
-        !make_map(&mBl, w_lo, 3, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B, 1, CU_TENSOR_MAP_DATA_TYPE_FLOAT16)) return DP_ERR_UNSUPPORTED;
+    cuuint64_t dims[3] = {Kp, (cuuint64_t)g.Nout, (cuuint64_t)l.T};
+    cuuint64_t str[2] = {Kp * 2, (cuuint64_t)g.Nout * Kp * 2};
+    cuuint32_t box[3] = {(cuuint32_t)BK, (cuuint32_t)PS_BN, 1};
+    if (!encode_map(&mBh, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, l.w_hi, 3, dims, str, box) ||
+        !encode_map(&mBl, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, l.w_lo, 3, dims, str, box)) return DP_ERR_UNSUPPORTED;
   }
   TcParams p{};
-  p.Nimg = Nimg; p.H = H; p.W = W; p.Nout = Nout;
-  p.ntaps = taps.n;
-  for (int i = 0; i < 9; ++i) { p.dh[i] = taps.dh[i]; p.dw[i] = taps.dw[i]; p.wt[i] = taps.wt[i]; }
-  p.os = os; p.oa = oa; p.ob = ob; p.Ho = Ho; p.Wo = Wo;
-  p.alpha = alpha; p.b_from_img = b_from_img; p.in_stride = in_stride; p.amax_a = amax_a; p.amax_b = amax_b; p.amax_out = amax_out;
-  p.kchunks = (Kg + BK - 1) / BK;
-  p.bw = bw; p.bh = bh; p.bn = bn; p.tiles_w = W / bw; p.tiles_h = H / bh;
-  p.y = out; p.ldy = ld_out; p.bias = bias; p.rowadd = rowadd; p.ld_rowadd = ld_rowadd; p.residual = residual; p.ld_res = ld_res;
-  p.accumulate = accumulate;
-  auto al16 = [](const void* q, long long ld) { return q == nullptr || ((((uintptr_t)q) & 15) == 0 && (ld % 4) == 0); };
-  p.vec4 = (al16(out, ld_out) && al16(bias, 0) && al16(rowadd, ld_rowadd) && al16(residual, ld_res)) ? 1 : 0;
-  const int tiles_n = (Nimg + bn - 1) / bn;
-  dim3 grid((unsigned)(p.tiles_w * p.tiles_h * tiles_n), (unsigned)((Nout + BN - 1) / BN));
-  p.ksplit = 1; p.it_per_split = p.ntaps * p.kchunks;
-  {
-    const int tiles_m = (int)grid.x, total = (int)(grid.x * grid.y);
-    if (ws && !b_from_img) {
-      p.ksplit = pick_ksplit(total, p.ntaps * p.kchunks, p.it_per_split);
-      p.ws = ws; p.ws_ld = (int)grid.y * 128; p.ws_split_stride = (long long)tiles_m * BM * p.ws_ld;
-    }
-    const int work = total * p.ksplit;
-    const int ctas = work < g_num_sms ? work : g_num_sms;
-    conv_tc_ps_kernel<false><<<ctas, THREADS, PS_SMEM, st>>>(mA, mBh, mBl, p, tiles_m, total);
-    if (p.ksplit > 1) {
-      int rc = dp_check_launch();
-      if (rc) return rc;
-      const long long items = (long long)tiles_m * BM * ((Nout + 3) / 4);
-      long long blocks = (items + 255) / 256;
-      if (blocks > g_num_sms * 8) blocks = g_num_sms * 8;
-      splitk_epilogue_kernel<<<(int)blocks, 256, 0, st>>>(p, tiles_m);
-    }
+  p.Nimg = g.N; p.H = g.H; p.W = g.W; p.Nout = g.Nout;
+  p.ntaps = g.taps.n;
+  for (int i = 0; i < 9; ++i) { p.dh[i] = g.taps.dh[i]; p.dw[i] = g.taps.dw[i]; p.wt[i] = g.taps.wt[i]; }
+  p.os = g.os; p.oa = g.oa; p.ob = g.ob; p.Ho = g.Ho; p.Wo = g.Wo;
+  p.alpha = l.alpha; p.b_from_img = l.b_from_img; p.in_stride = g.in_stride; p.amax_a = l.amax_a; p.amax_b = l.amax_b; p.amax_out = l.amax_out;
+  p.kchunks = (g.Kg + BK - 1) / BK;
+  p.bw = pl.bw; p.bh = pl.bh; p.bn = pl.bn; p.tiles_w = pl.tiles_w; p.tiles_h = pl.tiles_h;
+  p.y = l.out; p.ldy = l.ld_out; p.bias = l.bias; p.rowadd = l.rowadd; p.ld_rowadd = l.ld_rowadd; p.residual = l.residual; p.ld_res = l.ld_res;
+  p.accumulate = l.accumulate;
+  p.vec4 = (al16(l.out, l.ld_out) && al16(l.bias, 0) && al16(l.rowadd, l.ld_rowadd) && al16(l.residual, l.ld_res)) ? 1 : 0;
+  p.ksplit = pl.ksplit; p.it_per_split = pl.it_per_split;
+  if (split) { p.ws = l.ws; p.ws_ld = pl.n_tiles * PS_BN; p.ws_split_stride = (long long)pl.tiles_m * BM * p.ws_ld; }
+  if (any) {
+    const dp_conv_args* a = l.gather;
+    p.gx = l.act; p.gldx = l.ld_act; p.gH = a->H; p.gW = a->W; p.gC = a->C; p.gQ = a->Q; p.gPQ = a->P * a->Q; p.gS = a->S;
+    p.gstride = a->stride; p.gpad_t = a->pad_t; p.gpad_l = a->pad_l; p.gM = g.W; p.relu = (a->flags & DP_CONV_RELU) ? 1 : 0;
+  }
+  const int sms = runtime().num_sms, total = pl.tiles_m * pl.n_tiles, work = total * p.ksplit, ctas = work < sms ? work : sms;
+  if (any) conv_tc_ps_kernel<true><<<ctas, THREADS, PS_SMEM, st>>>(mBh, mBh, mBl, p, pl.tiles_m, total);
+  else conv_tc_ps_kernel<false><<<ctas, THREADS, PS_SMEM, st>>>(mA, mBh, mBl, p, pl.tiles_m, total);
+  if (p.ksplit > 1) {
+    const int rc = dp_check_launch();
+    if (rc) return rc;
+    const long long items = (any ? (long long)g.W : (long long)pl.tiles_m * BM) * ((g.Nout + 3) / 4);   // workspace rows x float4
+    long long blocks = (items + 255) / 256;
+    if (blocks > sms * 8) blocks = sms * 8;
+    if (any) splitk_flat_epilogue_kernel<<<(int)blocks, 256, 0, st>>>(p);
+    else splitk_epilogue_kernel<<<(int)blocks, 256, 0, st>>>(p, pl.tiles_m);
   }
   return dp_check_launch();
 }
@@ -927,7 +865,7 @@ extern "C" int dp_split_h3(const float* x, int64_t ld, int64_t bs, int32_t batch
     const int pitch = (cols + 7) & ~7;
     const int vec = ((((uintptr_t)x) & 15) == 0 && ld % 4 == 0 && bs % 4 == 0) ? 1 : 0;
     long long blocks = ((long long)rows * (pitch >> 3) + 255) / 256;
-    if (blocks > g_num_sms * 8) blocks = g_num_sms * 8;
+    if (blocks > runtime().num_sms * 8) blocks = runtime().num_sms * 8;
     split_h3_rows_kernel<<<dim3((unsigned)blocks, (unsigned)batch), 256, 0, (cudaStream_t)stream>>>(x, ld, bs, rows, cols, pitch, vec, (__half*)hi,
                                                                                                 (__half*)lo, amax);
   } else {
@@ -950,215 +888,105 @@ extern "C" int dp_transpose_batched(const float* in, float* out, int32_t batch, 
 extern "C" int dp_gemm_nt_tc(const dp_gemm_nt_args* a, dp_stream_t stream) {
   DP_REQUIRE(a && a->A && a->b_hi && a->b_lo && a->C, DP_ERR_NULL);
   DP_REQUIRE(a->batch > 0 && a->H > 0 && a->W > 0 && a->Kg > 0 && a->N > 0 && a->ld_a >= a->Kg && a->ldc >= a->N, DP_ERR_SHAPE);
-  if (a->batch > 127) { /* the B "tap" index travels in a signed char table only for real taps; images use n0 directly */ }
-  TapTable t{};
-  t.n = 1;
-  return launch_tc(a->A, a->ld_a, a->amax_a, a->batch, a->H, a->W, a->Kg, a->b_hi, a->b_lo, a->amax_b, a->N, a->batch, t, 1, 0, 0, a->H,
-                   a->W, a->C, a->ldc, nullptr, nullptr, 0, nullptr, 0, 0, (cudaStream_t)stream, a->alpha, 1, 1, (a->Kg + 7) & ~7, nullptr,
-                   nullptr, a->amax_out);
+  const ConvGemm g = {TapTable{1}, a->batch, a->H, a->W, a->Kg, a->N, 1, 0, 0, a->H, a->W, 1};
+  return launch_tc(g, {.act = a->A, .ld_act = a->ld_a, .amax_a = a->amax_a, .w_hi = a->b_hi, .w_lo = a->b_lo, .amax_b = a->amax_b,
+                       .T = a->batch, .ldb = (a->Kg + 7) & ~7, .out = a->C, .ld_out = a->ldc, .amax_out = a->amax_out, .alpha = a->alpha,
+                       .b_from_img = 1},
+                   (cudaStream_t)stream);
 }
 
 int dp_tc_runtime_ok() { return tc_init(); }
 
-static TapTable dense_taps(int R, int S, int pad, bool flip) {
-  TapTable t{};
-  t.n = R * S;
-  for (int r = 0; r < R; ++r)
-    for (int s = 0; s < S; ++s) {
-      int i = r * S + s;
-      t.dh[i] = (signed char)(r - pad); t.dw[i] = (signed char)(s - pad);
-      t.wt[i] = (signed char)(flip ? (R * S - 1 - i) : i);
-    }
-  return t;
-}
-
 int dp_conv2d_fprop_tc(const dp_conv_args* a, dp_stream_t stream) {
   if (!a || !a->x || !a->y) return DP_ERR_UNSUPPORTED;   // let the SIMT entry produce the precise error
   if (a->flags & DP_CONV_RELU) return DP_ERR_UNSUPPORTED;  // the ReLU epilogue lives on the SIMT kernel
-  if (a->R != a->S || (a->R != 1 && a->R != 3) || a->pad_l != a->pad_t) return DP_ERR_UNSUPPORTED;
-  // stride 1: 'same' padding.  stride 2: 3x3 with pad 1, or pad 0 + the (0,1,0,1) zero border of Downsample2D (resnet.py:213-218) which
-  // TMA out-of-bounds zero fill provides for free
-  if (!((a->stride == 1 && a->pad_t == (a->R - 1) / 2) || (a->stride == 2 && a->R == 3 && (a->pad_t == 0 || a->pad_t == 1)))) return DP_ERR_UNSUPPORTED;
-  if (a->P * a->stride != a->H || a->Q * a->stride != a->W) return DP_ERR_UNSUPPORTED;   // stride 2: even extents, out = in / 2 (Downsample2D, pad 1)
+  if (!box_geometry(a)) return DP_ERR_UNSUPPORTED;
   if (a->N <= 0 || a->H <= 0 || a->W <= 0 || a->C <= 0 || a->K <= 0 || a->ldx < a->C || a->ldy < a->K) return DP_ERR_UNSUPPORTED;
-  return launch_tc((const float*)a->x, a->ldx, a->amax_x, a->N, a->P, a->Q, a->C, a->w_tc_hi, a->w_tc_lo, a->amax_w, a->K, a->R * a->S,
-                   dense_taps(a->R, a->S, a->pad_t, false), 1, 0, 0, a->P, a->Q, (float*)a->y, a->ldy, a->bias, a->rowadd,
-                   a->ld_rowadd, a->residual, a->ld_res, (a->flags & DP_CONV_ACCUMULATE) ? 1 : 0, (cudaStream_t)stream, 1.0f, 0, a->stride, -1,
-                   a->workspace, nullptr, a->amax_out);
+  ConvGemm g[4];
+  conv_gemms(a, 0, g);
+  return launch_tc(g[0], conv_launch(a, false), (cudaStream_t)stream);
 }
 
 // General-geometry fprop (DP_CONV_ANY_GEOMETRY): any R x S, stride 1 or 2, explicit top / left padding, any N x H x W, on
 // conv_tc_ps_kernel<true>.  Channel counts below ANY_MIN_C stay on the SIMT kernel: a stage holds 64 input channels, and with fewer than 32
-// of them most of every 3 x fp16 product multiplies zero fill (Inception's C = 3 stem).  ws_need: geometry-only workspace query.
+// of them most of every 3 x fp16 product multiplies zero fill (Inception's C = 3 stem).  Its one GEMM runs over the [N][P][Q] output
+// pixels flattened into a [1][1][M] grid; the kernel walks the taps arithmetically.
 constexpr int ANY_MIN_C = 32;
-int fprop_tc_any(const dp_conv_args* a, float* ws, long long* ws_need, cudaStream_t st) {
+int any_gemm(const dp_conv_args* a, ConvGemm& g) {
   if (a->N <= 0 || a->H <= 0 || a->W <= 0 || a->C <= 0 || a->K <= 0 || a->P <= 0 || a->Q <= 0 || a->R <= 0 || a->S <= 0) return DP_ERR_UNSUPPORTED;
   if (a->C < ANY_MIN_C || (a->stride != 1 && a->stride != 2) || a->pad_t < 0 || a->pad_l < 0 || a->rowadd) return DP_ERR_UNSUPPORTED;
   if ((long long)a->N * a->P * a->Q >= (1ll << 31) || (long long)a->R * a->S > 65535) return DP_ERR_UNSUPPORTED;
-  if (!tc_init()) return DP_ERR_UNSUPPORTED;
-  const int M = a->N * a->P * a->Q, tiles_m = (M + BM - 1) / BM, n_tiles = (a->K + PS_BN - 1) / PS_BN;
-  const int kchunks = (a->C + BK - 1) / BK, iters = a->R * a->S * kchunks;
-  if (ws_need) {
-    int ips;
-    const int ks = pick_ksplit(tiles_m * n_tiles, iters, ips);
-    *ws_need = ks > 1 ? (long long)ks * tiles_m * BM * n_tiles * PS_BN : 0;
-    return DP_OK;
-  }
-  if (!a->x || !a->y || !a->w_tc_hi || !a->w_tc_lo || !a->amax_x || !a->amax_w) return DP_ERR_UNSUPPORTED;
-  if (a->ldx % 4 || ((uintptr_t)a->x & 15) || ((uintptr_t)a->w_tc_hi & 15) || ((uintptr_t)a->w_tc_lo & 15)) return DP_ERR_UNSUPPORTED;
-  CUtensorMap mBh, mBl;
-  {
-    const cuuint64_t Kp = (cuuint64_t)wrow(a->C);
-    cuuint64_t dims[3] = {Kp, (cuuint64_t)a->K, (cuuint64_t)(a->R * a->S)};
-    cuuint64_t str[2] = {Kp * 2, (cuuint64_t)a->K * Kp * 2};
-    cuuint32_t box[3] = {(cuuint32_t)BK, (cuuint32_t)PS_BN, 1};
-    if (!make_map(&mBh, a->w_tc_hi, 3, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B, 1, CU_TENSOR_MAP_DATA_TYPE_FLOAT16) ||
-        !make_map(&mBl, a->w_tc_lo, 3, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B, 1, CU_TENSOR_MAP_DATA_TYPE_FLOAT16)) return DP_ERR_UNSUPPORTED;
-  }
-  TcParams p{};
-  p.Nimg = 1; p.H = 1; p.W = M; p.Nout = a->K;
-  p.ntaps = a->R * a->S; p.kchunks = kchunks;
-  p.os = 1; p.oa = 0; p.ob = 0; p.Ho = 1; p.Wo = M;
-  p.alpha = 1.0f; p.b_from_img = 0; p.in_stride = 1; p.amax_a = a->amax_x; p.amax_b = a->amax_w; p.amax_out = a->amax_out;
-  p.bw = BM; p.bh = 1; p.bn = 1; p.tiles_w = tiles_m; p.tiles_h = 1;
-  p.y = (float*)a->y; p.ldy = a->ldy; p.bias = a->bias; p.residual = a->residual; p.ld_res = a->ld_res;
-  p.accumulate = (a->flags & DP_CONV_ACCUMULATE) ? 1 : 0;
-  auto al16 = [](const void* q, long long ld) { return q == nullptr || ((((uintptr_t)q) & 15) == 0 && (ld % 4) == 0); };
-  p.vec4 = (al16(a->y, a->ldy) && al16(a->bias, 0) && al16(a->residual, a->ld_res)) ? 1 : 0;
-  p.gx = (const float*)a->x; p.gldx = a->ldx; p.gH = a->H; p.gW = a->W; p.gC = a->C; p.gQ = a->Q; p.gPQ = a->P * a->Q; p.gS = a->S;
-  p.gstride = a->stride; p.gpad_t = a->pad_t; p.gpad_l = a->pad_l; p.gM = M; p.relu = (a->flags & DP_CONV_RELU) ? 1 : 0;
-  const int total = tiles_m * n_tiles;
-  p.ksplit = 1; p.it_per_split = iters;
-  if (ws) {
-    p.ksplit = pick_ksplit(total, iters, p.it_per_split);
-    p.ws = ws; p.ws_ld = n_tiles * PS_BN; p.ws_split_stride = (long long)tiles_m * BM * p.ws_ld;
-  }
-  const int work = total * p.ksplit;
-  conv_tc_ps_kernel<true><<<work < g_num_sms ? work : g_num_sms, THREADS, PS_SMEM, st>>>(mBh, mBh, mBl, p, tiles_m, total);
-  if (p.ksplit > 1) {
-    int rc = dp_check_launch();
-    if (rc) return rc;
-    long long blocks = ((long long)M * ((a->K + 3) / 4) + 255) / 256;
-    if (blocks > g_num_sms * 8) blocks = g_num_sms * 8;
-    splitk_flat_epilogue_kernel<<<(int)blocks, 256, 0, st>>>(p);
-  }
-  return dp_check_launch();
+  const int M = a->N * a->P * a->Q;
+  g = {TapTable{a->R * a->S}, 1, 1, M, a->C, a->K, 1, 0, 0, 1, M, 1};
+  return DP_OK;
 }
 int dp_conv2d_fprop_tc_any(const dp_conv_args* a, dp_stream_t stream) {
-  if (!a) return DP_ERR_UNSUPPORTED;
-  return fprop_tc_any(a, a->workspace, nullptr, (cudaStream_t)stream);
+  ConvGemm g;
+  if (!a || any_gemm(a, g) != DP_OK || !a->x || !a->y) return DP_ERR_UNSUPPORTED;
+  TcLaunch l = conv_launch(a, false);
+  l.gather = a;
+  return launch_tc(g, l, (cudaStream_t)stream);
 }
 
-// stride-1 dgrad == fprop of dy with the taps flipped and the (K,C) roles swapped: dx[n,h,w,c] = sum dy[n,h+1-r,w+1-s,k] W[k,c,r,s].
-// stride-2 dgrad: dx[2i+a, 2j+b] only sees taps with (a+pad-r), (b+pad-s) even -> 4 parity classes, each a dense GEMM over the
-// dy grid with 1/2/2/4 taps and a strided output mapping (no MACs wasted on structural zeros).
 int dp_conv2d_dgrad_tc(const dp_conv_args* a, dp_stream_t stream) {
   if (!a || !a->x || !a->y) return DP_ERR_UNSUPPORTED;
   if (a->N <= 0 || a->H <= 0 || a->W <= 0 || a->C <= 0 || a->K <= 0 || a->ldx < a->C || a->ldy < a->K) return DP_ERR_UNSUPPORTED;
-  if (a->R != a->S || (a->R != 1 && a->R != 3)) return DP_ERR_UNSUPPORTED;
-  const int acc = (a->flags & DP_CONV_ACCUMULATE) ? 1 : 0;
-  if (a->stride == 1) {
-    if (a->pad_t != (a->R - 1) / 2 || a->pad_l != a->pad_t || a->P != a->H || a->Q != a->W) return DP_ERR_UNSUPPORTED;
-    return launch_tc((const float*)a->y, a->ldy, a->amax_y, a->N, a->H, a->W, a->K, a->w_tc_hi, a->w_tc_lo, a->amax_w, a->C, a->R * a->S,
-                     dense_taps(a->R, a->S, a->pad_t, true), 1, 0, 0, a->H, a->W, (float*)a->x, a->ldx, nullptr, nullptr, 0, nullptr, 0,
-                     acc, (cudaStream_t)stream, 1.0f, 0, 1, -1, a->workspace, nullptr, a->amax_out);
+  // stride 2 takes any padding: the parity classes place every tap
+  if (a->stride == 1 ? !box_geometry(a) : !(a->stride == 2 && a->R == 3 && a->S == 3 && a->H == 2 * a->P && a->W == 2 * a->Q))
+    return DP_ERR_UNSUPPORTED;
+  ConvGemm g[4];
+  const int n = conv_gemms(a, 1, g);
+  const TcLaunch l = conv_launch(a, true);
+  for (int c = 0; c < n; ++c) {
+    const int rc = launch_tc(g[c], l, (cudaStream_t)stream);
+    // once a class has written dx the SIMT kernel cannot take over
+    if (rc != DP_OK) return (c == 0 || rc != DP_ERR_UNSUPPORTED) ? rc : DP_ERR_SHAPE;
   }
-  if (a->stride != 2 || a->R != 3 || a->H != 2 * a->P || a->W != 2 * a->Q) return DP_ERR_UNSUPPORTED;
-  TapTable cls[4];
-  for (int ca = 0; ca < 2; ++ca)
-    for (int cb = 0; cb < 2; ++cb) {
-      TapTable& t = cls[ca * 2 + cb];
-      t = TapTable{};
-      for (int r = 0; r < 3; ++r)
-        for (int s = 0; s < 3; ++s) {
-          int nh = ca + a->pad_t - r, nw = cb + a->pad_l - s;
-          if ((nh & 1) || (nw & 1)) continue;
-          t.dh[t.n] = (signed char)(nh / 2); t.dw[t.n] = (signed char)(nw / 2); t.wt[t.n] = (signed char)(r * 3 + s);
-          ++t.n;
-        }
-      if (t.n == 0) return DP_ERR_UNSUPPORTED;
-    }
-  for (int ca = 0; ca < 2; ++ca)
-    for (int cb = 0; cb < 2; ++cb) {
-      int rc = launch_tc((const float*)a->y, a->ldy, a->amax_y, a->N, a->P, a->Q, a->K, a->w_tc_hi, a->w_tc_lo, a->amax_w, a->C, 9, cls[ca * 2 + cb], 2, ca, cb,
-                         a->H, a->W, (float*)a->x, a->ldx, nullptr, nullptr, 0, nullptr, 0, acc, (cudaStream_t)stream, 1.0f, 0, 1, -1,
-                         a->workspace, nullptr, a->amax_out);
-      if (rc != DP_OK) return (ca == 0 && cb == 0) ? rc : (rc == DP_ERR_UNSUPPORTED ? DP_ERR_SHAPE : rc);
-    }
   return DP_OK;
 }
 
 // Floats of split-K workspace dp_conv2d_fprop (op 0) / dp_conv2d_dgrad (op 1) can use for this geometry (0: the launch fills the SMs
 // without splitting).  With a->workspace == NULL the launch simply does not split.
 extern "C" long long dp_conv_splitk_workspace_floats(const dp_conv_args* a, int op) {
+  TcPlan pl;
   if (a && op == 0 && (a->flags & DP_CONV_ANY_GEOMETRY)) {   // the box kernel's need, or else the general-geometry kernel's
     dp_conv_args b = *a;
     b.flags &= ~DP_CONV_ANY_GEOMETRY;
-    long long need = (a->flags & DP_CONV_RELU) ? 0 : dp_conv_splitk_workspace_floats(&b, 0), any = 0;
-    if (fprop_tc_any(a, nullptr, &any, nullptr) == DP_OK && any > need) need = any;
+    long long need = (a->flags & DP_CONV_RELU) ? 0 : dp_conv_splitk_workspace_floats(&b, 0);
+    ConvGemm g;
+    if (any_gemm(a, g) == DP_OK && plan_tc(g, true, true, pl) == DP_OK && pl.ws_floats > need) need = pl.ws_floats;
     return need;
   }
   if (!a || a->N <= 0 || a->H <= 0 || a->W <= 0 || a->C <= 0 || a->K <= 0 || a->R != a->S || (a->R != 1 && a->R != 3)) return 0;
   long long need = 0;
-  TapTable t{};
-  if (op == 0) {
-    t.n = a->R * a->S;
-    launch_tc(nullptr, 0, nullptr, a->N, a->P, a->Q, a->C, nullptr, nullptr, nullptr, a->K, t.n, t, 1, 0, 0, a->P, a->Q, nullptr, 0, nullptr,
-              nullptr, 0, nullptr, 0, 0, nullptr, 1.0f, 0, a->stride, -1, nullptr, &need);
-  } else if (a->stride == 1) {
-    t.n = a->R * a->S;
-    launch_tc(nullptr, 0, nullptr, a->N, a->H, a->W, a->K, nullptr, nullptr, nullptr, a->C, t.n, t, 1, 0, 0, a->H, a->W, nullptr, 0, nullptr,
-              nullptr, 0, nullptr, 0, 0, nullptr, 1.0f, 0, 1, -1, nullptr, &need);
-  } else {
-    for (int taps = 1; taps <= 4; taps *= 2) {     // the parity classes of a stride-2 3x3 dgrad have 1 / 2 / 2 / 4 taps and run back to back
-      long long n = 0;
-      t.n = taps;
-      launch_tc(nullptr, 0, nullptr, a->N, a->P, a->Q, a->K, nullptr, nullptr, nullptr, a->C, 9, t, 2, 0, 0, a->H, a->W, nullptr, 0, nullptr,
-                nullptr, 0, nullptr, 0, 0, nullptr, 1.0f, 0, 1, -1, nullptr, &n);
-      if (n > need) need = n;
-    }
-  }
+  ConvGemm g[4];
+  for (int c = 0, n = conv_gemms(a, op, g); c < n; ++c)      // the parity classes of a stride-2 dgrad run back to back
+    if (plan_tc(g[c], false, true, pl) == DP_OK && pl.ws_floats > need) need = pl.ws_floats;
   return need;
-}
-
-// 64-pixel K-chunk box of an [N][H][W] grid
-static bool pick_box64(int H, int W, int& bw, int& bh, int& bn) {
-  if (W >= WG_KPIX) { if (W % WG_KPIX) return false; bw = WG_KPIX; bh = 1; bn = 1; return true; }
-  if (WG_KPIX % W) return false;
-  bw = W;
-  int rem = WG_KPIX / W;
-  if (H >= rem) { if (H % rem) return false; bh = rem; bn = 1; return true; }
-  if (rem % H) return false;
-  bh = H; bn = rem / H;
-  return true;
 }
 
 int dp_conv2d_wgrad_tc(const dp_conv_args* a, dp_stream_t stream) {
   if (!a || !a->x || !a->y || !a->workspace) return DP_ERR_UNSUPPORTED;
   if (!tc_init()) return DP_ERR_UNSUPPORTED;
-  if (a->R != a->S || (a->R != 1 && a->R != 3) || a->pad_l != a->pad_t) return DP_ERR_UNSUPPORTED;
-  // stride 1: 'same' padding.  stride 2: 3x3 with pad 1, or pad 0 + the (0,1,0,1) zero border of Downsample2D (resnet.py:213-218) which
-  // TMA out-of-bounds zero fill provides for free
-  if (!((a->stride == 1 && a->pad_t == (a->R - 1) / 2) || (a->stride == 2 && a->R == 3 && (a->pad_t == 0 || a->pad_t == 1)))) return DP_ERR_UNSUPPORTED;
-  if (a->P * a->stride != a->H || a->Q * a->stride != a->W || a->splits < 1) return DP_ERR_UNSUPPORTED;
+  if (!box_geometry(a) || a->splits < 1) return DP_ERR_UNSUPPORTED;
   if (a->ldx % 4 || a->ldy % 4 || ((uintptr_t)a->x & 15) || ((uintptr_t)a->y & 15)) return DP_ERR_UNSUPPORTED;
   int bw, bh, bn;
   if (!a->amax_x || !a->amax_y) return DP_ERR_UNSUPPORTED;
-  if (!pick_box64(a->P, a->Q, bw, bh, bn)) return DP_ERR_UNSUPPORTED;   // 64-pixel chunks of the dy (output) grid; images past the batch
-  const int img_boxes = (a->N + bn - 1) / bn;                           // in the last box are TMA zero fill: they add nothing
+  if (!pick_box(WG_KPIX, a->P, a->Q, bw, bh, bn)) return DP_ERR_UNSUPPORTED;   // 64-pixel chunks of the dy (output) grid; images past
+  const int img_boxes = (a->N + bn - 1) / bn;                                   // the batch in the last box are TMA zero fill: they add nothing
   CUtensorMap mDy, mX;
   {
     cuuint64_t dims[4] = {(cuuint64_t)a->K, (cuuint64_t)a->Q, (cuuint64_t)a->P, (cuuint64_t)a->N};
     cuuint64_t str[3] = {(cuuint64_t)a->ldy * 4, (cuuint64_t)a->Q * a->ldy * 4, (cuuint64_t)a->P * a->Q * a->ldy * 4};
     cuuint32_t box[4] = {32, (cuuint32_t)bw, (cuuint32_t)bh, (cuuint32_t)bn};
-    if (!make_map(&mDy, a->y, 4, dims, str, box)) return DP_ERR_UNSUPPORTED;
+    if (!encode_map(&mDy, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, a->y, 4, dims, str, box)) return DP_ERR_UNSUPPORTED;
   }
   {   // x is sampled at stride * (output pixel) + tap offset: TMA element strides on W, H
     cuuint64_t dims[4] = {(cuuint64_t)a->C, (cuuint64_t)a->W, (cuuint64_t)a->H, (cuuint64_t)a->N};
     cuuint64_t str[3] = {(cuuint64_t)a->ldx * 4, (cuuint64_t)a->W * a->ldx * 4, (cuuint64_t)a->H * a->W * a->ldx * 4};
     cuuint32_t box[4] = {32, (cuuint32_t)(bw * a->stride), (cuuint32_t)(bh * a->stride), (cuuint32_t)bn};
     if (box[1] > 256 || box[2] > 256) return DP_ERR_UNSUPPORTED;
-    if (!make_map(&mX, a->x, 4, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B, a->stride)) return DP_ERR_UNSUPPORTED;
+    if (!encode_map(&mX, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, a->x, 4, dims, str, box, a->stride)) return DP_ERR_UNSUPPORTED;
   }
   WgParams p{};
   p.Nimg = a->N; p.H = a->P; p.W = a->Q; p.C = a->C; p.K = a->K; p.R = a->R; p.S = a->S; p.pad = a->pad_t; p.in_stride = a->stride;
@@ -1186,7 +1014,7 @@ extern "C" int dp_pack_conv_weight_tc(const float* w, int32_t K, int32_t C, int3
   const int Cp = wrow(C), Kp = wrow(K);
   long long total = (long long)R * S * ((long long)K * Cp > (long long)C * Kp ? (long long)K * Cp : (long long)C * Kp);
   int blocks = (int)((total + 255) / 256);
-  if (blocks > g_num_sms * 16) blocks = g_num_sms * 16;
+  if (blocks > runtime().num_sms * 16) blocks = runtime().num_sms * 16;
   pack_tc_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(w, K, C, R * S, Cp, Kp, (__half*)kc_hi, (__half*)kc_lo, (__half*)ck_hi, (__half*)ck_lo,
                                                            amax_w);
   return dp_check_launch();

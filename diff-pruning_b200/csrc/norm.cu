@@ -617,9 +617,6 @@ __global__ void __launch_bounds__(NT, 4) gn_bwd_apply4_kernel(const dp_gn_args a
   if (a.amax_dx) amax_commit(a.amax_dx, amax);
 }
 
-
-static inline bool al16(const void* p, long long ld) { return p == nullptr || ((((uintptr_t)p) & 15) == 0 && (ld % 4) == 0); }
-
 // ------------------------------------------------------------------------------------------------------------
 // LayerNorm = GroupNorm with ONE group over the channels of a ONE-pixel "image" (the LDM transformer blocks call it on every token:
 // N = tokens).  The chunked kernels above would spend a whole 256-thread block on one token; here a warp owns a row: float4 loads,

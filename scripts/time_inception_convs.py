@@ -23,7 +23,7 @@ GEOMS = [(128, 128, 1, 7, 1, 0, 3, 17, 17, 13), (160, 192, 7, 1, 1, 3, 0, 17, 17
 
 
 def box_takes(N, H, W, C, R, S, st, ph, pw, P, Q):
-    """The shapes dp_conv2d_fprop's box tensor-core kernel accepts (conv_tc.cu: dp_conv2d_fprop_tc, pick_box)."""
+    """The shapes dp_conv2d_fprop's box tensor-core kernel accepts (conv_tc.cu: dp_conv2d_fprop_tc; sm90_host.cuh: box_geometry, pick_box)."""
     if R != S or R not in (1, 3) or ph != pw or C % 4:
         return False
     if not ((st == 1 and ph == (R - 1) // 2) or (st == 2 and R == 3 and ph in (0, 1))) or P * st != H or Q * st != W:
