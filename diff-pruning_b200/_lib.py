@@ -122,6 +122,7 @@ _SIGS = {
     "dp_sumsq": (C.c_int, [vp, i64, vp, vp, vp]),
     "dp_adam_clip_ema": (C.c_int, [C.POINTER(AdamArgs), vp]),
     "dp_ddim_step": (C.c_int, [vp, vp, vp, vp, i64, f32, f32, f32, f32, f32, f32, vp]),
+    "dp_ddim_cfg_step": (C.c_int, [vp, i64, vp, vp, vp, vp, i64, vp, i32, i32, i32, i32, i32, f32, f32, f32, f32, f32, f32, vp]),
     "dp_scale": (C.c_int, [vp, i64, f32, vp]),
     "dp_fid_input": (C.c_int, [vp, i32, i32, i32, i32, i32, vp, i64, i32, i32, i32, i32, vp, vp]),
     "dp_pool3x3": (C.c_int, [vp, i64, vp, i64, i32, i32, i32, i32, i32, i32, i32, vp, vp]),

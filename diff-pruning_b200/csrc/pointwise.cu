@@ -266,15 +266,51 @@ __global__ void softmax_bwd_kernel(const float* __restrict__ p, const float* __r
     }
   }
 }
+// The DDIM update of one element, shared by both samplers: x0 = (x - sb e) / sa, then sap x0 + dir e (+ sigma nz).  kRn: every operation
+// rounded on its own (no fma contraction), in the order torch evaluates p_sample_ddim (ddim.py:194-202), so the result is bit-identical to
+// that fp32 torch code; otherwise the compiler may contract, as dp_ddim_step always has.
+template <bool kRn>
+__device__ __forceinline__ float ddim_x0(float x, float e, float sb, float sa) {
+  if (kRn) return __fdiv_rn(__fsub_rn(x, __fmul_rn(sb, e)), sa);
+  return (x - sb * e) / sa;
+}
+template <bool kRn>
+__device__ __forceinline__ float ddim_prev(float x0, float e, float sap, float dir, bool has_nz, float sigma, float nz) {
+  if (kRn) {
+    float v = __fadd_rn(__fmul_rn(sap, x0), __fmul_rn(dir, e));
+    return has_nz ? __fadd_rn(v, __fmul_rn(sigma, nz)) : v;
+  }
+  float v = sap * x0 + dir * e;
+  if (has_nz) v += sigma * nz;
+  return v;
+}
 __global__ void ddim_step_kernel(const float* __restrict__ x, const float* __restrict__ eps, const float* __restrict__ nz,
                                  float* __restrict__ out, long long n, float sb, float sa, float clip, float sap, float dir, float sigma) {
   for (long long i = blockIdx.x * (long long)NT + threadIdx.x; i < n; i += (long long)gridDim.x * NT) {
     float e = eps[i];
-    float x0 = (x[i] - sb * e) / sa;
+    float x0 = ddim_x0<false>(x[i], e, sb, sa);
     if (clip > 0.f) x0 = fminf(fmaxf(x0, -clip), clip);
-    float v = sap * x0 + dir * e;
-    if (nz) v += sigma * nz[i];
-    out[i] = v;
+    out[i] = ddim_prev<false>(x0, e, sap, dir, nz != nullptr, sigma, nz ? nz[i] : 0.f);
+  }
+}
+// Guided DDIM step of the LDM sampler over the NCHW state x [B][C][HW]: eps_hat is read from the UNet's NHWC output (pixel stride ld_eps),
+// images 0..B-1 unconditional and B..2B-1 conditional when guided (e = e_u + s (e_c - e_u)), images 0..B-1 as is otherwise.  x_prev goes
+// to x_out (NCHW) and to the UNet's NHWC input (pixel stride ld_in), into both halves when guided; pred_x0 (NCHW) when asked for.
+__global__ void ddim_cfg_step_kernel(const float* __restrict__ eps, long long ld_eps, const float* __restrict__ x, const float* __restrict__ nz,
+                                     float* __restrict__ x_out, float* __restrict__ x_in, long long ld_in, float* __restrict__ pred_x0,
+                                     int B, int C, int HW, int guided, float scale, float sb, float sa, float sap, float dir, float sigma) {
+  const long long n = (long long)B * C * HW, half_eps = (long long)B * HW * ld_eps, half_in = (long long)B * HW * ld_in;
+  for (long long i = blockIdx.x * (long long)NT + threadIdx.x; i < n; i += (long long)gridDim.x * NT) {
+    const int c = (int)((i / HW) % C);
+    const long long pix = (i / ((long long)C * HW)) * HW + i % HW;       // image * HW + pixel
+    float e = eps[pix * ld_eps + c];
+    if (guided) e = __fadd_rn(e, __fmul_rn(scale, __fsub_rn(eps[half_eps + pix * ld_eps + c], e)));
+    const float x0 = ddim_x0<true>(x[i], e, sb, sa);
+    const float v = ddim_prev<true>(x0, e, sap, dir, nz != nullptr, sigma, nz ? nz[i] : 0.f);
+    x_out[i] = v;
+    x_in[pix * ld_in + c] = v;
+    if (guided) x_in[half_in + pix * ld_in + c] = v;
+    if (pred_x0) pred_x0[i] = x0;
   }
 }
 __global__ void scale_kernel(float* __restrict__ x, long long n, float s) {
@@ -402,6 +438,18 @@ extern "C" int dp_ddim_step(const float* x, const float* eps, const float* noise
   DP_REQUIRE(sigma == 0.f || noise, DP_ERR_NULL);
   ddim_step_kernel<<<nblocks(n, NT), NT, 0, (cudaStream_t)st>>>(x, eps, sigma != 0.f ? noise : nullptr, out, n, sqrt_beta_t, sqrt_alpha_t,
                                                               clip, sqrt_alpha_prev, dir_coef, sigma);
+  return dp_check_launch();
+}
+extern "C" int dp_ddim_cfg_step(const float* eps, int64_t ld_eps, const float* x, const float* noise, float* x_out, float* x_in, int64_t ld_in,
+                                float* pred_x0, int32_t B, int32_t C, int32_t H, int32_t W, int32_t guided, float scale,
+                                float sqrt_one_minus_at, float sqrt_at, float sqrt_a_prev, float dir_coef, float sigma, dp_stream_t st) {
+  DP_REQUIRE(eps && x && x_out && x_in, DP_ERR_NULL);
+  DP_REQUIRE(B > 0 && C > 0 && H > 0 && W > 0 && ld_eps >= C && ld_in >= C && sqrt_at > 0.f, DP_ERR_SHAPE);
+  DP_REQUIRE(sigma == 0.f || noise, DP_ERR_NULL);
+  const long long n = (long long)B * C * H * W;
+  ddim_cfg_step_kernel<<<nblocks(n, NT), NT, 0, (cudaStream_t)st>>>(eps, ld_eps, x, sigma != 0.f ? noise : nullptr, x_out, x_in, ld_in, pred_x0,
+                                                                  B, C, H * W, guided ? 1 : 0, scale, sqrt_one_minus_at, sqrt_at, sqrt_a_prev,
+                                                                  dir_coef, sigma);
   return dp_check_launch();
 }
 extern "C" int dp_scale(float* x, int64_t n, float s, dp_stream_t st) {

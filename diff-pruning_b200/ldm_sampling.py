@@ -1,0 +1,445 @@
+"""prune_ldm.py's sample-then-score loop (BASELINE configs[4], ldm_exp/prune_ldm.py:105-131) on the engine, in latent space.
+
+ClassEmbedder    — ldm/modules/encoders/modules.py:21-33 (`embedding.weight`), the cin256-v2 conditioning (1001 classes, 1000 = unconditional).
+LatentDiffusion  — a thin container of what the loop uses of ldm/models/diffusion/ddpm.py's LatentDiffusion: `model.diffusion_model` (the
+                   UNetModel of ldm.py), `cond_stage_model`, the schedule buffers, get_learned_conditioning / apply_model / get_loss_at_t,
+                   and load_state_dict of a Lightning checkpoint's `state_dict`.  Not a Lightning module; no first stage, no EMA.
+DDIMSampler      — ldm/models/diffusion/ddim.py: the same `sample(...)` call and results.  The whole S-step sample is ONE CUDA graph: per
+                   step a fill of the timestep, the no-grad plan's forward at batch 2B (unconditional | conditional), and dp_ddim_cfg_step,
+                   which forms the guided eps, writes x_prev and feeds both halves of the next forward's input.
+LDMPruneScorer   — the loop itself: classes -> guided DDIM-20 sample -> get_loss_at_t at t = iteration on the samples with fresh noise ->
+                   the stop rule of --pruner diff-pruning / diff0 -> backward into the UNet's gradient arena.
+
+Gradients reach the UNet only: the reference's trainable ClassEmbedder also gets a gradient from loss.backward(), but the pruner looks at
+`diffusion_model` alone, and the context enters the engine as a constant input.
+"""
+from __future__ import annotations
+
+import random
+from types import SimpleNamespace
+from typing import Callable, Dict, List, Optional, Sequence
+
+import numpy as np
+import torch
+import torch.nn as nn
+
+from . import _lib as L
+from .engine import _stream, frozen_weights, get_plan
+from .ldm import CIN256_V2_CONFIG, UNetModel
+from .scoring import TaylorScorer
+
+
+class ClassEmbedder(nn.Module):
+    """modules.py:21-33: batch[key] (B,) class labels -> (B, 1, embed_dim)."""
+
+    def __init__(self, embed_dim: int, n_classes: int = 1001, key: str = "class_label"):
+        super().__init__()
+        self.key = key
+        self.embedding = nn.Embedding(n_classes, embed_dim)
+
+    def forward(self, batch, key=None):
+        return self.embedding(batch[self.key if key is None else key][:, None])
+
+
+class DiffusionWrapper(nn.Module):
+    """ddpm.py DiffusionWrapper with conditioning_key 'crossattn': holds `diffusion_model` (the state-dict prefix `model.diffusion_model.`)."""
+
+    def __init__(self, diffusion_model: UNetModel):
+        super().__init__()
+        self.diffusion_model = diffusion_model
+        self.conditioning_key = "crossattn"
+
+    def forward(self, x, t, c_crossattn=None):
+        return self.diffusion_model(x, t, context=torch.cat(list(c_crossattn), 1))
+
+
+def make_ddim_timesteps(num_ddim_timesteps: int, num_ddpm_timesteps: int = 1000) -> np.ndarray:
+    """util.py make_ddim_timesteps, 'uniform': range(0, T, T // S) + 1."""
+    c = num_ddpm_timesteps // num_ddim_timesteps
+    return np.asarray(list(range(0, num_ddpm_timesteps, c))) + 1
+
+
+def ddim_schedule(alphas_cumprod: torch.Tensor, S: int, eta: float) -> SimpleNamespace:
+    """DDIMSampler.make_schedule's DDIM arrays (ddim.py:24-53, util.py make_ddim_sampling_parameters) in the dtypes the reference ends up
+    with: alphas = float32 table entries, alphas_prev = float64 array of float32 values, sigmas = float64 (eta times the float64 square root
+    of a mix of float64 and float32 terms; pinned bit for bit by tests/test_ldm_sampling_host.py), sqrt(1 - alphas) in float32.  `coefs[index]` are the fp32 scalars p_sample_ddim forms from them
+    (ddim.py:190-202): (sqrt(1 - a_t), sqrt(a_t), sqrt(a_prev), sqrt(1 - a_prev - sigma^2), sigma)."""
+    ac = alphas_cumprod.detach().to("cpu", torch.float32)
+    ts = make_ddim_timesteps(S, ac.shape[0])
+    alphas = ac[ts]
+    alphas_prev = np.asarray([float(ac[0])] + ac[ts[:-1]].tolist())
+    ap64 = torch.from_numpy(alphas_prev)
+    # (1 - alphas_prev) / (1 - alphas) is ndarray / float32 tensor, which torch evaluates as the float32 reciprocal of the divisor
+    # times the float64 numerator; alphas / alphas_prev is float32 / float64, a float64 quotient
+    sigmas = eta * torch.sqrt((1 - alphas).reciprocal().double() * (1 - ap64) * (1 - alphas.double() / ap64))
+    sqrt_one_minus = torch.sqrt(1. - alphas)
+    f32 = lambda v: torch.tensor([float(v)], dtype=torch.float32)        # torch.full((b, 1, 1, 1), v): a float32 fill
+    coefs = []
+    for i in range(S):
+        a_t, a_prev, sigma_t, sb = f32(alphas[i]), f32(alphas_prev[i]), f32(sigmas[i]), f32(sqrt_one_minus[i])
+        coefs.append((float(sb), float(a_t.sqrt()), float(a_prev.sqrt()), float((1. - a_prev - sigma_t ** 2).sqrt()), float(sigma_t)))
+    return SimpleNamespace(ddim_timesteps=ts, ddim_alphas=alphas, ddim_alphas_prev=alphas_prev, ddim_sigmas=sigmas,
+                           ddim_sqrt_one_minus_alphas=sqrt_one_minus, coefs=coefs)
+
+
+class _MSELoss(torch.autograd.Function):
+    """mean((out - target)^2) and its gradient 2 (out - target) / n from one dp_mse_loss_grad launch (the kernel of the fast path)."""
+
+    @staticmethod
+    def forward(ctx, out, target):
+        lib = L.load()
+        o, tg = out.contiguous(), target.contiguous()
+        n = o.numel()
+        grad = torch.empty_like(o)
+        loss = torch.zeros(1, device=o.device, dtype=torch.float32)
+        partial = torch.empty(max(1, lib.dp_mse_partials(n)), device=o.device, dtype=torch.float32)
+        L.check(lib.dp_mse_loss_grad(o.data_ptr(), tg.data_ptr(), grad.data_ptr(), n, 1.0 / n, 2.0 / n, partial.data_ptr(),
+                                     loss.data_ptr(), _stream()), "mse")
+        ctx.save_for_backward(grad)
+        return loss[0]
+
+    @staticmethod
+    def backward(ctx, gout):
+        grad, = ctx.saved_tensors
+        return grad * gout, None
+
+
+class LatentDiffusion(nn.Module):
+    """What prune_ldm.py uses of ldm/models/diffusion/ddpm.py's LatentDiffusion at the cin256-v2 settings (eps parameterisation, l2 loss,
+    l_simple_weight 1, logvar 0, original_elbo_weight 0, linear schedule 0.0015..0.0195 over 1000 steps, class-label cross-attention)."""
+
+    def __init__(self, unet_config: Optional[dict] = None, cond_stage_config: Optional[dict] = None, timesteps: int = 1000,
+                 linear_start: float = 0.0015, linear_end: float = 0.0195, cond_stage_key: str = "class_label"):
+        super().__init__()
+        self.model = DiffusionWrapper(UNetModel(**(unet_config or CIN256_V2_CONFIG)))
+        self.cond_stage_model = ClassEmbedder(**(cond_stage_config or dict(embed_dim=512, n_classes=1001, key=cond_stage_key)))
+        self.cond_stage_key = cond_stage_key
+        self.parameterization = "eps"
+        self.num_timesteps = timesteps
+        # ddpm.py:117-145: float64 schedule, stored as float32
+        betas = torch.linspace(linear_start ** 0.5, linear_end ** 0.5, timesteps, dtype=torch.float64) ** 2
+        ac = torch.cumprod(1.0 - betas, dim=0)
+        self.register_buffer("betas", betas.float())
+        self.register_buffer("alphas_cumprod", ac.float())
+        self.register_buffer("alphas_cumprod_prev", torch.cat([torch.ones(1, dtype=torch.float64), ac[:-1]]).float())
+
+    @property
+    def device(self):
+        return self.betas.device
+
+    def load_state_dict(self, state_dict, strict: bool = True):
+        """A Lightning checkpoint's `state_dict` (prune_ldm.py:21-28): `model.diffusion_model.*`, `cond_stage_model.*` and the three
+        schedule buffers are loaded; `first_stage_model.*` (the VQ-f4 autoencoder), `model_ema.*` and the schedule buffers this container
+        does not hold are ignored."""
+        own = set(self.state_dict().keys())
+        keep = {k: v for k, v in state_dict.items()
+                if k.startswith(("model.diffusion_model.", "cond_stage_model.")) or (k in own and "." not in k)}
+        return super().load_state_dict(keep, strict=strict)
+
+    def get_learned_conditioning(self, c):
+        """ddpm.py get_learned_conditioning with the ClassEmbedder: {cond_stage_key: (B,) labels} -> (B, 1, embed_dim)."""
+        return self.cond_stage_model(c)
+
+    def apply_model(self, x_noisy, t, cond):
+        """ddpm.py:901-924 for crossattn conditioning: the UNet with context = cond (a tensor, or a list / {'c_crossattn': [...]}).
+        The context is a constant of the engine's forward (no gradient flows into it)."""
+        if isinstance(cond, dict):
+            cond = cond["c_crossattn"]
+        if isinstance(cond, (list, tuple)):
+            cond = torch.cat(list(cond), 1)
+        return self.model.diffusion_model(x_noisy, t, context=cond.detach())
+
+    def q_sample(self, x_start, t, noise):
+        """ddpm.py:275-278 on the device (dp_add_noise: sqrt of the float32 alphas_cumprod entry, within an ulp of the reference's
+        float32-rounded float64 square roots; the fast path uses the same kernel)."""
+        x, nz = x_start.contiguous(), noise.contiguous()
+        out = torch.empty_like(x)
+        B, C_, H, W = x.shape
+        tt = t.to(device=x.device, dtype=torch.int64).contiguous()
+        acp = self.alphas_cumprod.to(x.device).contiguous()
+        L.check(L.load().dp_add_noise(x.data_ptr(), nz.data_ptr(), tt.data_ptr(), acp.data_ptr(), out.data_ptr(), B, C_, H, W, 0, 0,
+                                      _stream()), "add_noise")
+        return out
+
+    def get_loss_at_t(self, x, c, t, noise=None):
+        """ddpm.py:881-889 -> p_losses (:1022-1056) at the cin256-v2 values: the mean over C, H, W per image, then over the batch, of
+        (eps_hat - noise)^2 — one mean over all elements, as one kernel forms it with its gradient.  With logvar 0 and
+        original_elbo_weight 0 the other terms add exactly 0.  Returns (loss, loss_dict) like the reference."""
+        if isinstance(c, dict):
+            c = self.get_learned_conditioning(c)
+        noise = torch.randn_like(x) if noise is None else noise
+        if not torch.is_tensor(t):
+            t = torch.full((x.shape[0],), int(t), dtype=torch.long, device=x.device)
+        out = self.apply_model(self.q_sample(x.detach(), t, noise), t, c)
+        loss = _MSELoss.apply(out, noise)
+        prefix = "train" if self.training else "val"
+        return loss, {f"{prefix}/loss_simple": loss.detach(), f"{prefix}/loss": loss.detach()}
+
+
+class DDIMSampler:
+    """ldm/models/diffusion/ddim.py on the engine (uniform discretisation, eta, classifier-free guidance).
+
+    x_T (when not given) and the sigma noise are drawn with torch.randn on `generator` (the default generator of the device when None):
+    x_T first, then one (B, C, H, W) draw per step.  With eta == 0 no per-step noise is drawn; the reference draws it and multiplies it by
+    zero, so after an eta-0 sample the random stream is where the reference's is not."""
+
+    def __init__(self, model: LatentDiffusion, schedule: str = "linear", **kwargs):
+        self.model = model
+        self.ddpm_num_timesteps = model.num_timesteps
+        self.schedule = schedule
+        self.use_graph = True
+        self._graphs: Dict[tuple, SimpleNamespace] = {}
+        self.last_run: Optional[SimpleNamespace] = None    # static buffers of the last sample: every step's x_prev / pred_x0
+
+    def make_schedule(self, ddim_num_steps, ddim_discretize="uniform", ddim_eta=0., verbose=True):
+        if ddim_discretize != "uniform":
+            raise NotImplementedError(f"ddim_discretize={ddim_discretize!r}: only the uniform DDIM discretisation is on the engine")
+        sch = ddim_schedule(self.model.alphas_cumprod, ddim_num_steps, ddim_eta)
+        for k, v in vars(sch).items():
+            setattr(self, k, v)
+
+    @torch.no_grad()
+    def sample(self, S, batch_size, shape, conditioning=None, callback=None, normals_sequence=None, img_callback=None, quantize_x0=False,
+               eta=0., mask=None, x0=None, temperature=1., noise_dropout=0., score_corrector=None, corrector_kwargs=None, verbose=True,
+               x_T=None, log_every_t=100, unconditional_guidance_scale=1., unconditional_conditioning=None, generator=None, **kwargs):
+        """ddim.py:55-104 + ddim_sampling (:106-163): returns (samples, {'x_inter': [...], 'pred_x0': [...]}) with x_T first and the
+        steps whose index % log_every_t == 0 or index == S - 1 after it."""
+        unsupported = {"mask / x0": mask is not None or x0 is not None, "quantize_x0": quantize_x0, "score_corrector": score_corrector is not None,
+                       "temperature != 1": temperature != 1., "noise_dropout": noise_dropout > 0., "callback / img_callback":
+                       callback is not None or img_callback is not None, "ddim_use_original_steps": kwargs.get("ddim_use_original_steps", False),
+                       "ddim_discretize != uniform": kwargs.get("ddim_discretize", "uniform") != "uniform"}
+        bad = [k for k, v in unsupported.items() if v]
+        if bad:
+            raise NotImplementedError(f"DDIMSampler options outside prune_ldm's sampling: {bad}")
+        if not torch.is_tensor(conditioning):
+            raise NotImplementedError("conditioning must be the (B, 1, context_dim) tensor get_learned_conditioning returns")
+        self.make_schedule(S, ddim_eta=eta, verbose=verbose)
+        unet = self.model.model.diffusion_model
+        dev = unet.device
+        if dev.type != "cuda":
+            raise RuntimeError("diff_pruning_b200: DDIMSampler samples on a CUDA device (no CPU fallback)")
+        C_, H, W = shape
+        B = batch_size
+        guided = unconditional_conditioning is not None and unconditional_guidance_scale != 1.
+        gdev = generator.device if generator is not None else dev
+        if x_T is None:
+            x_T = torch.randn((B, C_, H, W), generator=generator, device=gdev, dtype=torch.float32)
+        was_training = unet.training
+        unet.eval()
+        try:
+            frozen = unet.__dict__.get("_dpb200_frozen", False)
+            with (_nullctx() if frozen else frozen_weights(unet)):
+                plan = get_plan(unet, 2 * B if guided else B, H, W, dev, need_grad=False)
+                plan.ensure_packed()
+                run = self._run_for(plan, S, float(eta), float(unconditional_guidance_scale), guided, B, C_, H, W)
+                run.x_T.copy_(x_T.to(dev, torch.float32).reshape(B, C_, H, W))
+                ctx = conditioning.reshape(B, 1, -1)
+                if guided:
+                    ctx = torch.cat([unconditional_conditioning.reshape(B, 1, -1).to(ctx.device), ctx])
+                plan.load_context(ctx)
+                if run.noise is not None:
+                    for i in range(S):
+                        run.noise[i].copy_(torch.randn((B, C_, H, W), generator=generator, device=gdev, dtype=torch.float32))
+                if run.graph is not None:
+                    run.graph.replay()
+                else:
+                    run.body()
+        finally:
+            unet.train(was_training)
+        self.last_run = run
+        inter = {"x_inter": [run.x_T.clone()], "pred_x0": [run.x_T.clone()]}
+        for i in range(S):
+            index = S - i - 1
+            if index % log_every_t == 0 or index == S - 1:
+                inter["x_inter"].append(run.xs[i].clone())
+                inter["pred_x0"].append(run.x0s[i].clone())
+        return run.xs[S - 1].clone(), inter
+
+    def _run_for(self, plan, S, eta, scale, guided, B, C_, H, W) -> SimpleNamespace:
+        """The static buffers and the captured graph of one (plan, S, eta, scale), built on first use."""
+        key = (id(plan), S, eta, scale, guided, self.use_graph)
+        run = self._graphs.get(key)
+        if run is not None and run.plan is plan:
+            return run
+        lib, dev = L.load(), plan.dev
+        run = SimpleNamespace(plan=plan, graph=None)
+        run.x_T = torch.empty((B, C_, H, W), device=dev, dtype=torch.float32)
+        run.xs = torch.empty((S, B, C_, H, W), device=dev, dtype=torch.float32)      # x_prev of step i
+        run.x0s = torch.empty((S, B, C_, H, W), device=dev, dtype=torch.float32)     # pred_x0 of step i
+        run.noise = torch.empty((S, B, C_, H, W), device=dev, dtype=torch.float32) if eta > 0 else None
+        steps = [(int(step), S - i - 1) for i, step in enumerate(np.flip(self.ddim_timesteps))]
+        coefs = list(self.coefs)
+        x_in, y_out = plan.x_in, plan.y_out
+        half_in = B * H * W * x_in.ld * 4
+
+        def body():
+            s = _stream()
+            L.check(lib.dp_nchw_to_nhwc(run.x_T.data_ptr(), x_in.ptr, x_in.ld, B, C_, H, W, s), "x_T nchw->nhwc")
+            if guided:
+                L.check(lib.dp_nchw_to_nhwc(run.x_T.data_ptr(), x_in.ptr + half_in, x_in.ld, B, C_, H, W, s), "x_T nchw->nhwc")
+            for i, (step, index) in enumerate(steps):
+                plan.t_dev.fill_(step)
+                plan.run_forward(s)
+                sb, sa, sap, dirc, sigma = coefs[index]
+                x = run.x_T if i == 0 else run.xs[i - 1]
+                nz = run.noise[i].data_ptr() if (run.noise is not None and sigma != 0.) else None
+                L.check(lib.dp_ddim_cfg_step(y_out.ptr, y_out.ld, x.data_ptr(), nz, run.xs[i].data_ptr(), x_in.ptr, x_in.ld,
+                                             run.x0s[i].data_ptr(), B, C_, H, W, 1 if guided else 0, scale, sb, sa, sap, dirc, sigma, s),
+                        "ddim_cfg_step")
+        run.body = body
+        if self.use_graph:
+            run.x_T.zero_()
+            if run.noise is not None:
+                run.noise.zero_()
+            torch.cuda.synchronize(dev)
+            side = torch.cuda.Stream(device=dev)
+            side.wait_stream(torch.cuda.current_stream(dev))
+            with torch.cuda.stream(side):      # warm-up outside capture (lazy module loading)
+                body()
+            torch.cuda.current_stream(dev).wait_stream(side)
+            torch.cuda.synchronize(dev)
+            g = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(g):
+                body()
+            run.graph = g
+        self._graphs[key] = run
+        return run
+
+
+class _nullctx:
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        return False
+
+
+PRUNE_LDM_THRESHOLDS = {"taylor": None, "diff-pruning": 0.1, "diff0": 0.0}
+
+
+class PruneLDMStopRule:
+    """prune_ldm.py:120-131: max_loss (starting at -1) is updated FIRST, then `diff-pruning` (0.1) / `diff0` (0.0) stop when
+    loss / max_loss < thr, BEFORE loss.backward() — the stopping iteration's gradient is not accumulated.  `taylor` never stops.
+    The quotient and the comparison are fp32, as on the reference's 0-dim fp32 tensors."""
+
+    def __init__(self, pruner: str):
+        if pruner not in PRUNE_LDM_THRESHOLDS:
+            raise ValueError(f"pruner must be one of {sorted(PRUNE_LDM_THRESHOLDS)}, got {pruner!r}")
+        self.thr = PRUNE_LDM_THRESHOLDS[pruner]
+        self.max_loss = np.float32(-1.0)
+
+    def stop(self, loss: float) -> bool:
+        l32 = np.float32(loss)
+        if l32 > self.max_loss:
+            self.max_loss = l32
+        if self.thr is None:
+            return False
+        with np.errstate(divide="ignore", invalid="ignore"):
+            return bool(np.float32(l32 / self.max_loss) < np.float32(self.thr))
+
+
+class LDMPruneScorer:
+    """The fast path of prune_ldm.py:105-131: per iteration t = 0, 1, ...: B random classes (`class_sampler(B)`, by default
+    random.sample(range(1000), B) on the module-level `random` as the script does), their context, a guided DDIM sample of B latents
+    (DDIMSampler: one graph replay), then get_loss_at_t(samples, t, fresh noise) as two graphs — forward + loss, whose loss is read back
+    to the host for the stop rule, and the backward, which accumulates into the UNet's Parameter.grad (the plan's gradient arena)."""
+
+    def __init__(self, model: LatentDiffusion, n_samples_per_class: int = 6, ddim_steps: int = 20, scale: float = 3.0, eta: float = 0.0,
+                 use_graph: bool = True):
+        self.model = model
+        self.B, self.S, self.scale, self.eta = n_samples_per_class, ddim_steps, float(scale), float(eta)
+        self.unet = model.model.diffusion_model
+        self.dev = self.unet.device
+        cfg = self.unet.config
+        self.shape = (cfg.in_channels, cfg.image_size, cfg.image_size)
+        self.use_graph = use_graph
+        self.sampler = DDIMSampler(model)
+        self.sampler.use_graph = use_graph
+        self.ts: Optional[TaylorScorer] = None
+        self.g_fwd = self.g_bwd = None
+        self.stopped_at: Optional[int] = None
+
+    def _labels(self, class_sampler) -> torch.Tensor:
+        labels = class_sampler(self.B) if class_sampler is not None else random.sample(range(1000), self.B)
+        return torch.as_tensor(labels, dtype=torch.long).to(self.dev)
+
+    def _scorer(self, samples, noise, c) -> TaylorScorer:
+        if self.ts is None:
+            self.ts = TaylorScorer(self.unet, samples, noise, alphas_cumprod=self.model.alphas_cumprod, use_graph=False, context=c)
+        else:
+            self.ts.clean.copy_(samples)
+            self.ts.noise.copy_(noise)
+            self.ts.plan.load_context(c)
+        return self.ts
+
+    def _fwd(self):
+        self.ts._refresh_noise()
+        self.ts._forward_loss()
+
+    def _bwd(self):
+        self.ts.plan.run_backward(_stream())
+
+    def _capture(self):
+        ts, dev = self.ts, self.dev
+        torch.cuda.synchronize(dev)
+        side = torch.cuda.Stream(device=dev)
+        side.wait_stream(torch.cuda.current_stream(dev))
+        with torch.cuda.stream(side):       # warm-up outside capture (lazy module loading); the gradient arena is restored after it
+            saved = ts.plan.grad_arena.clone()
+            self._fwd()
+            self._bwd()
+            ts.plan.grad_arena.copy_(saved)
+        torch.cuda.current_stream(dev).wait_stream(side)
+        torch.cuda.synchronize(dev)
+        self.g_fwd, self.g_bwd = torch.cuda.CUDAGraph(), torch.cuda.CUDAGraph()
+        with torch.cuda.graph(self.g_fwd):
+            self._fwd()
+        with torch.cuda.graph(self.g_bwd):
+            self._bwd()
+
+    def run(self, pruner: str = "taylor", iterations: int = 1000, class_sampler: Optional[Callable[[int], Sequence[int]]] = None,
+            generator: Optional[torch.Generator] = None) -> torch.Tensor:
+        """The loop of prune_ldm.py:105-131 for `pruner` in {taylor, diff-pruning, diff0}.  Returns the losses of the iterations that
+        ran (with the stopping one last when the rule stopped the loop, its gradient not accumulated; self.stopped_at is its index)."""
+        rule = PruneLDMStopRule(pruner)
+        model, B = self.model, self.B
+        key = model.cond_stage_key
+        gdev = generator.device if generator is not None else self.dev
+        losses: List[float] = []
+        self.stopped_at = None
+        was_training = self.unet.training
+        self.unet.eval()                     # prune_ldm.py:72
+        try:
+            with torch.no_grad(), frozen_weights(self.unet):
+                uc = model.get_learned_conditioning({key: torch.full((B,), 1000, dtype=torch.long, device=self.dev)})
+                for t in range(iterations):
+                    labels = self._labels(class_sampler)
+                    c = model.get_learned_conditioning({key: labels})
+                    samples, _ = self.sampler.sample(S=self.S, conditioning=c, batch_size=B, shape=list(self.shape), verbose=False,
+                                                     unconditional_guidance_scale=self.scale, unconditional_conditioning=uc, eta=self.eta,
+                                                     generator=generator)
+                    noise = torch.randn(samples.shape, generator=generator, device=gdev, dtype=torch.float32).to(self.dev)
+                    ts = self._scorer(samples, noise, c)
+                    p = ts.plan
+                    p.check_current()
+                    p.attach_grads()
+                    p.ensure_packed()
+                    p.t_dev.fill_(t)
+                    if self.use_graph:
+                        if self.g_fwd is None:
+                            self._capture()
+                        self.g_fwd.replay()
+                    else:
+                        self._fwd()
+                    loss = float(ts.loss.item())
+                    losses.append(loss)
+                    if rule.stop(loss):
+                        self.stopped_at = t
+                        break
+                    if self.use_graph:
+                        self.g_bwd.replay()
+                    else:
+                        self._bwd()
+        finally:
+            self.unet.train(was_training)
+        return torch.tensor(losses, dtype=torch.float32)

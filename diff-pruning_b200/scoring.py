@@ -53,7 +53,8 @@ class TaylorScorer:
         self.plan: Plan = get_plan(model, B, H, W, self.dev, need_grad=True, fused_scores=fused_scores)
         if was_training:
             model.train()
-        if hasattr(self.plan, "ctx_in"):      # latent-diffusion UNetModel: cross-attention conditioning, fixed for the whole loop (prune_ldm.py:106-122)
+        if hasattr(self.plan, "ctx_in"):      # latent-diffusion UNetModel: cross-attention conditioning.  prune_ldm.py:105-131 draws new
+            # classes, hence a new context (and new latents), every iteration: ldm_sampling.LDMPruneScorer reloads it with plan.load_context
             if context is None:
                 raise ValueError("the LDM UNetModel needs context=(B, 1, context_dim)")
             self.plan.load_context(context)
@@ -74,7 +75,8 @@ class TaylorScorer:
         L.check(self.lib.dp_nchw_to_nhwc(self.noise.data_ptr(), self.noise_nhwc.data_ptr(), self.noise_nhwc.shape[-1], self.B, self.C,
                                          self.H, self.W, _stream()), "noise nchw->nhwc")
 
-    def _body(self):
+    def _forward_loss(self):
+        """add_noise -> forward -> loss and its gradient d loss / d y_out: everything of a pass up to the backward."""
         lib, p, s = self.lib, self.plan, _stream()
         L.check(lib.dp_add_noise(self.clean.data_ptr(), self.noise.data_ptr(), p.t_dev.data_ptr(), self.acp.data_ptr(),
                                  p.x_in.ptr, self.B, self.C, self.H, self.W, 1, p.x_in.ld, s), "add_noise")
@@ -82,7 +84,10 @@ class TaylorScorer:
         gy = p.gradof(p.y_out)
         L.check(lib.dp_mse_loss_grad(p.y_out.ptr, self.noise_nhwc.data_ptr(), gy.ptr, self.n, self.loss_scale, self.grad_scale,
                                      self.partial.data_ptr(), self.loss.data_ptr(), s), "mse")
-        p.run_backward(s)
+
+    def _body(self):
+        self._forward_loss()
+        self.plan.run_backward(_stream())
 
     def _capture(self):
         torch.cuda.synchronize(self.dev)

@@ -353,6 +353,18 @@ int dp_adam_clip_ema(const dp_adam_args* a, dp_stream_t stream);
 int dp_ddim_step(const float* x, const float* eps, const float* noise, float* out, int64_t n, float sqrt_beta_t, float sqrt_alpha_t,
                  float clip, float sqrt_alpha_prev, float dir_coef, float sigma, dp_stream_t stream);
 
+/* One step of the latent-diffusion DDIM sampler with classifier-free guidance (ldm/models/diffusion/ddim.py:165-202, temperature 1, no
+ * score corrector / quantisation / noise dropout), over the NCHW fp32 state x [B][C][H][W]:
+ *   guided:  e = e_u + scale * (e_c - e_u), e_u / e_c = images 0..B-1 / B..2B-1 of eps (the UNet output at batch 2B for cat([uc, c]))
+ *   else:    e = images 0..B-1 of eps (a batch-B UNet output)
+ *   x0 = (x - sqrt_one_minus_at * e) / sqrt_at ;  x_prev = sqrt_a_prev * x0 + dir_coef * e (+ sigma * noise)
+ * eps and x_in are NHWC with pixel strides ld_eps / ld_in.  Each operation is separately rounded in that order (no fma contraction), so
+ * for the same eps the result equals fp32 torch bit for bit.  x_prev is written to x_out (NCHW, not aliasing x) and to x_in (both halves,
+ * images i and B+i, when guided: the next forward's input); x0 to pred_x0 (NCHW) unless NULL; noise (NCHW) may be NULL when sigma == 0. */
+int dp_ddim_cfg_step(const float* eps, int64_t ld_eps, const float* x, const float* noise, float* x_out, float* x_in, int64_t ld_in,
+                     float* pred_x0, int32_t B, int32_t C, int32_t H, int32_t W, int32_t guided, float scale, float sqrt_one_minus_at,
+                     float sqrt_at, float sqrt_a_prev, float dir_coef, float sigma, dp_stream_t stream);
+
 /* y[i] = x[i] * s  (gradient averaging after all-reduce etc.) */
 int dp_scale(float* x, int64_t n, float s, dp_stream_t stream);
 

@@ -16,6 +16,7 @@ Outputs (all small, committed):
     tests/golden/ddim_tiny.pt      DDIMPipeline samples (uniform/eta 0/10 steps, quad/eta 0.5/7 steps) on TINY
     tests/golden/fid_*             FID Inception fixtures (gen_fid): weight-file layout, features of seeded weights, Frechet cases
     tests/golden/ssim_ref.pt       SSIM fixtures (gen_ssim): uint8 image pairs and utils_image.py's per-channel / per-image SSIM
+    tests/golden/ldm_ddim_tiny.pt  guided DDIM sampling of the tiny LDM by ldm_exp's DDIMSampler, every step, and one get_loss_at_t pass
 """
 import argparse
 import hashlib
@@ -526,6 +527,130 @@ def gen_ldm_tiny():
     print("ldm_tiny", losses, n_full, len(redrawn), os.path.getsize(os.path.join(OUT, "ldm_tiny.pt")))
 
 
+LDM_DDIM_RUNS = [(S, scale, eta) for S in (4, 20) for scale in (1.0, 3.0) for eta in (0.0, 0.5)]
+
+
+def gen_ldm_ddim():
+    """prune_ldm.py's sample-then-score loop on the tiny LDM (tests/golden/ldm_ddim_tiny.pt), from the UNMODIFIED reference: its DDIMSampler
+    (ldm/models/diffusion/ddim.py, with register_buffer keeping the buffers on the CPU, ref_shim.cpu_ddim_sampler), its UNetModel (weights as
+    gen_ldm_tiny makes them) and its ClassEmbedder (ldm/modules/encoders/modules.py:21-33, seed 1) behind a shim with LatentDiffusion's
+    schedule buffers (ddpm.py:117-145, cin256-v2: linear 0.0015..0.0195, 1000 steps) and apply_model (crossattn context).
+    One 3 x 8 x 8 latent per sample (2 images per guided forward) (small enough to keep the file small; 64 / 16 tokens in the two transformer levels).  Per run
+    (S, scale, eta) with a fixed x_T and torch.manual_seed(20 + run) for the sigma noise: the DDIM timesteps and schedule arrays as
+    make_schedule leaves them (dtype included), the samples and the intermediates at log_every_t = 5; for the 4-step runs and the 20-step
+    scale-3 eta-0.5 run also every step's raw UNet output (the 2B batch when guided), x_prev and pred_x0.  Then one get_loss_at_t
+    (p_losses, ddpm.py:1022-1056, restated: eps, l2, logvar 0, no elbo term) at t = 5 on the S = 20, scale 3, eta 0 samples with seeded
+    noise: the loss, the UNet output, (sum, sum |g|, sum g^2) of every UNet gradient and its first 32 elements.  The embedding weights
+    are reproducible (seed 1): only their digest is stored."""
+    import functools
+    import numpy as np
+    ref_shim.install_ldm()
+    from ldm.modules.diffusionmodules.openaimodel import UNetModel as RefUNet
+    from ldm.modules.diffusionmodules.util import make_beta_schedule
+    from ldm.modules.encoders.modules import ClassEmbedder as RefClassEmbedder
+    from diff_pruning_b200 import ldm as L
+    cfg = dict(L.LDM_TINY_CONFIG)
+    torch.manual_seed(0)
+    unet = RefUNet(**cfg).eval()
+    g = torch.Generator().manual_seed(5)
+    for k, p in unet.named_parameters():
+        if float(p.detach().abs().sum()) == 0 and p.dim() > 1:
+            p.data.copy_(torch.randn(p.shape, generator=g) * 0.05)
+    torch.manual_seed(1)
+    emb = RefClassEmbedder(cfg["context_dim"], n_classes=1001, key="class_label")
+
+    class Shim:
+        """LatentDiffusion's attributes that DDIMSampler reads (ddpm.py:117-145 register_schedule, :901-924 apply_model)."""
+        num_timesteps, device = 1000, torch.device("cpu")
+
+        def __init__(self):
+            betas = make_beta_schedule("linear", 1000, linear_start=0.0015, linear_end=0.0195)
+            ac = np.cumprod(1. - betas, axis=0)
+            to_torch = functools.partial(torch.tensor, dtype=torch.float32)
+            self.betas, self.alphas_cumprod = to_torch(betas), to_torch(ac)
+            self.alphas_cumprod_prev = to_torch(np.append(1., ac[:-1]))
+            self.sqrt_alphas_cumprod, self.sqrt_one_minus_alphas_cumprod = to_torch(np.sqrt(ac)), to_torch(np.sqrt(1. - ac))
+            self.raw = []
+
+        def apply_model(self, x, t, cond):
+            out = unet(x, t, context=cond)
+            self.raw.append(out.detach().clone())
+            return out
+
+    shim = Shim()
+    Sampler = ref_shim.cpu_ddim_sampler()
+    B = 1
+    labels, ulabels = torch.tensor([998]), torch.tensor([1000])
+    with torch.no_grad():
+        c, uc = emb({"class_label": labels}), emb({"class_label": ulabels})
+    HW = 8
+    x_T = torch.randn(B, 3, HW, HW, generator=torch.Generator().manual_seed(7))
+
+    def arr(v):
+        return {"value": torch.as_tensor(np.asarray(v) if not torch.is_tensor(v) else v).clone(), "type": type(v).__name__,
+                "dtype": str(v.dtype)}
+
+    runs = {}
+    for k, (S, scale, eta) in enumerate(LDM_DDIM_RUNS):
+        steps = []
+
+        class Rec(Sampler):
+            def p_sample_ddim(self, x, c_, t, index, **kw):
+                n0 = len(shim.raw)
+                x_prev, pred_x0 = super().p_sample_ddim(x, c_, t, index, **kw)
+                if S == 4 or (scale, eta) == (3.0, 0.5):
+                    steps.append({"t": int(t[0]), "index": index, "raw": shim.raw[n0].clone(), "x_prev": x_prev.clone(),
+                                  "pred_x0": pred_x0.clone()})
+                return x_prev, pred_x0
+
+        sampler = Rec(shim)
+        torch.manual_seed(20 + k)
+        samples, inter = sampler.sample(S=S, batch_size=B, shape=[3, HW, HW], conditioning=c, verbose=False, eta=eta, x_T=x_T.clone(),
+                                        log_every_t=5, unconditional_guidance_scale=scale, unconditional_conditioning=uc)
+        sched = {n: arr(getattr(sampler, n)) for n in ("ddim_timesteps", "ddim_alphas", "ddim_alphas_prev", "ddim_sigmas",
+                                                       "ddim_sqrt_one_minus_alphas")}
+        # the per-step fp32 scalars p_sample_ddim forms (ddim.py:190-193: torch.full of one entry of each array)
+        full = {n: torch.tensor([float(torch.full((1,), getattr(sampler, a)[i]).item()) for i in range(S)], dtype=torch.float32)
+                for n, a in (("a_t", "ddim_alphas"), ("a_prev", "ddim_alphas_prev"), ("sigma_t", "ddim_sigmas"),
+                             ("sqrt_one_minus_at", "ddim_sqrt_one_minus_alphas"))}
+        x_inter = torch.stack(inter["x_inter"])
+        logged = [next(i for i, s in enumerate(steps) if torch.equal(s["x_prev"], v)) for v in x_inter[1:]] if steps else None
+        packed = {f: torch.stack([st[f] for st in steps]) for f in ("raw", "x_prev", "pred_x0")} if steps else None
+        if packed:                      # one stacked tensor per field: per-tensor records would outweigh the data
+            packed.update({f: torch.tensor([st[f] for st in steps]) for f in ("t", "index")})
+        runs[(S, scale, eta)] = {"seed": 20 + k, "sched": sched, "full": full, "steps": packed, "samples": samples.clone(),
+                                 "x_inter": x_inter, "logged_steps": logged}
+        shim.raw.clear()
+        print("ldm_ddim", S, scale, eta, float(samples.abs().max()), logged)
+
+    x0 = runs[(20, 3.0, 0.0)]["samples"]
+    noise = torch.randn(x0.shape, generator=torch.Generator().manual_seed(11))
+    t = torch.full((B,), 5, dtype=torch.long)
+    unet.zero_grad()
+    emb.zero_grad()
+    cond = emb({"class_label": labels})
+    ex = lambda a: a.gather(-1, t).reshape(B, 1, 1, 1)           # util.py extract_into_tensor
+    x_noisy = ex(shim.sqrt_alphas_cumprod) * x0 + ex(shim.sqrt_one_minus_alphas_cumprod) * noise
+    out = unet(x_noisy, t, context=cond)
+    loss = ((out - noise) ** 2).mean([1, 2, 3])
+    logvar_t = torch.zeros(1000)[t]
+    loss = 1.0 * (loss / torch.exp(logvar_t) + logvar_t).mean()
+    loss.backward()
+    torch.save({"cfg": cfg, "runs_keys": LDM_DDIM_RUNS, "runs": runs, "x_T": x_T, "labels": labels, "ulabels": ulabels,
+                "embedding_sha": hashlib.sha256(emb.embedding.weight.detach().numpy().tobytes()).hexdigest(),
+                "emb_keys": list(emb.state_dict().keys()),
+                "schedule": {"betas": shim.betas, "alphas_cumprod": shim.alphas_cumprod, "alphas_cumprod_prev": shim.alphas_cumprod_prev},
+                "loss_t": 5, "loss_noise": noise, "loss": float(loss), "loss_out": out.detach(),
+                "grad_names": [k for k, _ in unet.named_parameters()],
+                "grad_samples": torch.stack([torch.nn.functional.pad(p.grad.flatten()[:32], (0, max(0, 32 - p.numel())))
+                                             for p in unet.parameters()]),
+                "grad_numel": torch.tensor([p.numel() for p in unet.parameters()]),
+                "grad_fp": torch.tensor([fp(p.grad) for p in unet.parameters()], dtype=torch.float64),
+                "emb_grad_fp": fp(emb.embedding.weight.grad)},
+               os.path.join(OUT, "ldm_ddim_tiny.pt"))
+    print("ldm_ddim loss", float(loss), os.path.getsize(os.path.join(OUT, "ldm_ddim_tiny.pt")))
+
+
 def gen_ref_pickle():
     """A whole-module pickle exactly as the reference writes it (`torch.save(model)`, ddpm_prune.py:135) for a small member of the
     family after a `--pruner magnitude` prune at ratio 0.3 — default AttnProcessor2_0 objects, FrozenDict config and all — plus eps_hat
@@ -679,7 +804,7 @@ if __name__ == "__main__":
     ap.add_argument("--only", default=None)
     a = ap.parse_args()
     torch.set_num_threads(os.cpu_count())
-    jobs = {"ssim": gen_ssim, "fid": gen_fid,"ldm_tiny": gen_ldm_tiny, "exp_importance": gen_exp_importance, "ref_pickle": gen_ref_pickle, "lsun_struct": gen_lsun_struct, "lr": gen_lr, "ckpt": gen_ckpt, "ddim": gen_ddim, "tiny": gen_tiny, "blocks": gen_blocks, "finetune": gen_finetune, "cifar_fwd": gen_cifar_fwd,
+    jobs = {"ssim": gen_ssim, "fid": gen_fid,"ldm_tiny": gen_ldm_tiny, "ldm_ddim": gen_ldm_ddim, "exp_importance": gen_exp_importance, "ref_pickle": gen_ref_pickle, "lsun_struct": gen_lsun_struct, "lr": gen_lr, "ckpt": gen_ckpt, "ddim": gen_ddim, "tiny": gen_tiny, "blocks": gen_blocks, "finetune": gen_finetune, "cifar_fwd": gen_cifar_fwd,
             "cfg1_s3": gen_cfg1_s3, "cfg3_s3": gen_cfg3_s3, "cfg1": gen_cfg1}
     for name, fn in jobs.items():
         if a.only and name != a.only:

@@ -43,3 +43,28 @@ def install():
     import torch_pruning  # noqa: F401
 
     return diffusers, torch_pruning
+
+
+def install_ldm():
+    """Makes ldm_exp's `ldm` package importable on CPUs: omegaconf (openaimodel.py:476) and the text-encoder dependencies that
+    ldm/modules/encoders/modules.py imports at the top (clip, kornia) are stubbed; the classes used from these modules need none of them."""
+    sys.path.insert(0, os.path.join(REF, "ldm_exp"))
+    oc, lc = types.ModuleType("omegaconf"), types.ModuleType("omegaconf.listconfig")
+    lc.ListConfig = type("ListConfig", (list,), {})
+    oc.listconfig = lc
+    sys.modules.setdefault("omegaconf", oc)
+    sys.modules.setdefault("omegaconf.listconfig", lc)
+    for name in ("clip", "kornia"):
+        sys.modules.setdefault(name, types.ModuleType(name))
+
+
+def cpu_ddim_sampler():
+    """The reference's DDIMSampler (ldm/models/diffusion/ddim.py) with a register_buffer that leaves tensors on their device: the
+    original moves every tensor buffer to CUDA (ddim.py:18-22).  Everything else, the schedule and the sampling loop, is the unmodified
+    reference code."""
+    from ldm.models.diffusion.ddim import DDIMSampler
+
+    class CpuDDIMSampler(DDIMSampler):
+        def register_buffer(self, name, attr):
+            setattr(self, name, attr)
+    return CpuDDIMSampler
