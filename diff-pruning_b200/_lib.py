@@ -129,6 +129,8 @@ _SIGS = {
     "dp_global_mean": (C.c_int, [vp, i64, vp, i64, i32, i32, i32, i32, vp]),
     "dp_feature_moments": (C.c_int, [vp, i64, i64, i32, vp, vp, vp, vp]),
     "dp_ssim": (C.c_int, [C.POINTER(SsimArgs), vp]),
+    "dp_vq_quantize": (C.c_int, [vp, i32, i32, i32, i32, f32, vp, i32, i32, vp, i64, vp, vp]),
+    "dp_decode_images": (C.c_int, [vp, i64, i32, i32, i32, i32, vp, vp, vp]),
 }
 EXPORTS = tuple(_SIGS)
 

@@ -661,7 +661,9 @@ class Plan:
     def qkv_fusable(self, x: View, lins) -> bool:
         ws = [l.weight for l in lins]
         inner, Cin = ws[0].shape[0], ws[0].shape[1]
-        return bool(self.FUSE_QKV and self.tc and not self.bf16 and all(tuple(w.shape) == (inner, Cin) for w in ws)
+        # (inner, Cin) linear weights, or (inner, Cin, 1, 1) 1x1 convolution weights (the VQ decoder's AttnBlock): the same memory layout
+        return bool(self.FUSE_QKV and self.tc and not self.bf16 and all(tuple(w.shape[:2]) == (inner, Cin) and w.numel() == inner * Cin
+                                                                        for w in ws)
                     and inner * Cin >= 256 and x.rows >= 128 and len({l.bias is None for l in lins}) == 1)
 
     def conv_qkv(self, x: View, lins) -> Tuple[View, View, View]:
@@ -866,23 +868,26 @@ class Plan:
 
     # ------------------------------------------------------------------ blocks
     def resnet(self, m: ResnetBlock2D, x: View, out: View):
-        """ResnetBlock2D.forward — resnet.py:589-639."""
+        """ResnetBlock2D.forward — resnet.py:589-639.  A block without a time embedding (time_emb_proj None: the VQ decoder's
+        ResnetBlock, model.py:121-141 with temb None) skips the per-image row of conv1's epilogue."""
         assert m.output_scale_factor == 1.0, "output_scale_factor != 1 is outside the DDPM configs"
         Cout = m.conv1.out_channels
         p_drop = float(m.dropout.p) if (self.training and m.dropout.p > 0) else 0.0
         a1 = self.new(x.N, x.H, x.W, x.C)
         h1 = self.new(x.N, x.H, x.W, Cout)
         a2 = self.new(x.N, x.H, x.W, Cout)
-        tp = self.new(self.B, 1, 1, Cout)
+        has_temb = m.time_emb_proj is not None
+        tp = self.new(self.B, 1, 1, Cout) if has_temb else None
         has_sc = m.conv_shortcut is not None
         da = lambda: self.sptr("da")
         g1 = self.gn(x, m.norm1, a1, silu=True, bf16_only=self.conv_bf16_ok(a1, h1, m.conv1.weight))
         if self.need_grad:
             self.gn_bwd(g1, x, m.norm1, da, x.C, add2=None if has_sc else self.gradof(out))
-        # time_emb_proj(silu(temb)) -> per-image row added in conv1's epilogue; its dY are conv1's per-image sums
-        self.conv(self.silu_temb, m.time_emb_proj.weight, m.time_emb_proj.bias, tp, pad=0, dy_dense="seg",
-                  dx_into=self.silu_temb)
-        self.conv(a1, m.conv1.weight, m.conv1.bias, h1, rowadd=tp, seg_out="seg", dx_scratch="da")
+        if has_temb:
+            # time_emb_proj(silu(temb)) -> per-image row added in conv1's epilogue; its dY are conv1's per-image sums
+            self.conv(self.silu_temb, m.time_emb_proj.weight, m.time_emb_proj.bias, tp, pad=0, dy_dense="seg",
+                      dx_into=self.silu_temb)
+        self.conv(a1, m.conv1.weight, m.conv1.bias, h1, rowadd=tp, seg_out="seg" if has_temb else None, dx_scratch="da")
         g2 = self.gn(h1, m.norm2, a2, silu=True, dropout_p=p_drop, bf16_only=self.conv_bf16_ok(a2, out, m.conv2.weight))
         if self.need_grad:
             self.gn_bwd(g2, h1, m.norm2, da, Cout)
@@ -973,7 +978,9 @@ class Plan:
         lib = self.lib
         i8, t8 = (inner + 7) // 8 * 8, (T + 7) // 8 * 8
         nsplit = N * max(T * i8, inner * t8)          # fp16 elements; the scratch is counted in floats
-        self.scratch("att_hi", (nsplit + 1) // 2); self.scratch("att_lo", (nsplit + 1) // 2); self.scratch("att_t", N * T * T)
+        self.scratch("att_hi", (nsplit + 1) // 2); self.scratch("att_lo", (nsplit + 1) // 2)
+        if self.need_grad:      # P^T / dS^T of the backward (N T^2 floats: 512 MB for 8 images of 4096 tokens)
+            self.scratch("att_t", N * T * T)
         Pp = P.data_ptr()
 
         def split(lst, src: View, slot: int, transpose: int):   # src is an [N][T][inner] activation view
@@ -1096,6 +1103,8 @@ class Plan:
     def _build(self):
         if hasattr(self.model, "input_blocks"):      # latent-diffusion UNetModel (ldm.py)
             return self._build_ldm()
+        if hasattr(self.model, "post_quant_conv"):   # VQ first-stage decoder (autoencoder.py)
+            return self._build_vq_decoder()
         m = self.model
         H, W = self.H, self.W
         cfg = m.config
@@ -1382,6 +1391,71 @@ class Plan:
         c = context.reshape(self.B, -1).to(device=self.dev, dtype=torch.float32)
         assert c.shape[1] == self.ctx_in.C, (tuple(context.shape), self.ctx_in.C)
         self.ctx_in.t.view(self.B, -1)[:, :self.ctx_in.C].copy_(c, non_blocking=True)
+
+    # ------------------------------------------------------------------ VQ first-stage decoder (autoencoder.py; cin256-v2 first_stage_config)
+    def vq_attention(self, m, x: View, out: View):
+        """AttnBlock (model.py:150-202): GroupNorm(32, eps 1e-6) -> q, k, v as 1x1 convolutions -> softmax(q k^T * c^-0.5) v over the
+        H*W tokens -> 1x1 proj_out ; + x."""
+        N, H, W, Cc = x.N, x.H, x.W, x.C
+        xn = self.new(N, H, W, Cc)
+        self.gn(x, m.norm, xn, silu=False)
+        convs = (m.q, m.k, m.v)
+        if self.qkv_fusable(xn, convs):
+            q, k, v = self.conv_qkv(xn, convs)
+        else:
+            q, k, v = (self.new(N, H, W, c.out_channels) for c in convs)
+            for c, t in zip(convs, (q, k, v)):
+                self.conv(xn, c.weight, c.bias, t, pad=0)
+        o = self.new(N, H, W, v.C)
+        self._attn_core(q, k, v, o, float(int(Cc) ** -0.5))
+        self.conv(o, m.proj_out.weight, m.proj_out.bias, out, pad=0, residual=x)
+
+    def _build_vq_decoder(self):
+        """VQModelInterface.decode after the codebook lookup (autoencoder.py:279-281) and Decoder.forward (model.py:535-568) as a
+        forward-only plan: post_quant_conv -> conv_in -> mid (resnet, attention, resnet) -> per level, resnets (+ attention) and nearest x2
+        + 3x3 conv -> GroupNorm + SiLU -> conv_out.  B, H, W are the latent's; x_in (the quantised latent, written by dp_vq_quantize) and
+        y_out (the decoded images) are padded NHWC buffers."""
+        from types import SimpleNamespace as NS
+        if self.need_grad:
+            raise NotImplementedError("the VQ decoder plan is forward-only: build it with need_grad=False")
+        m = self.model
+        dec = m.decoder
+        B, H, W = self.B, self.H, self.W
+        self.grad_arena = torch.zeros(0, device=self.dev)
+        self.x_in = self._padded(B, H, W, m.post_quant_conv.in_channels)
+        z = self._padded(B, H, W, m.post_quant_conv.out_channels)       # conv_in's C = 3 operand: pad channels zero, as x_in's
+        self.conv(self.x_in, m.post_quant_conv.weight, m.post_quant_conv.bias, z, pad=0)
+        x = self.new(B, H, W, dec.conv_in.out_channels)
+        self.conv(z, dec.conv_in.weight, dec.conv_in.bias, x)
+
+        def resnet(rb, x: View) -> View:     # ResnetBlock (model.py:82-141) in the attribute vocabulary of Plan.resnet()
+            y = self.new(x.N, x.H, x.W, rb.out_channels)
+            self.resnet(NS(norm1=rb.norm1, conv1=rb.conv1, time_emb_proj=None, norm2=rb.norm2, dropout=rb.dropout, conv2=rb.conv2,
+                           conv_shortcut=getattr(rb, "nin_shortcut", None), output_scale_factor=1.0), x, y)
+            return y
+
+        def attention(ab, x: View) -> View:
+            y = self.new(x.N, x.H, x.W, x.C)
+            self.vq_attention(ab, x, y)
+            return y
+
+        x = resnet(dec.mid.block_2, attention(dec.mid.attn_1, resnet(dec.mid.block_1, x)))
+        for i_level in reversed(range(len(dec.up))):
+            lvl = dec.up[i_level]
+            for i_block, rb in enumerate(lvl.block):
+                x = resnet(rb, x)
+                if len(lvl.attn) > 0:
+                    x = attention(lvl.attn[i_block], x)
+            if i_level != 0:
+                u = lvl.upsample.conv
+                y = self.new(x.N, 2 * x.H, 2 * x.W, u.out_channels)
+                self.conv(self._upsample2x(x), u.weight, u.bias, y)
+                x = y
+        a = self.new(x.N, x.H, x.W, x.C)
+        self.gn(x, dec.norm_out, a, silu=True)
+        self.y_out = self._padded(B, x.H, x.W, dec.conv_out.out_channels)
+        self.conv(a, dec.conv_out.weight, dec.conv_out.bias, self.y_out)
+        self._finalize_build()
 
     # ------------------------------------------------------------------ execution
     def run_pack(self, s: Optional[int] = None):

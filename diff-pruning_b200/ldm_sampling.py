@@ -3,19 +3,24 @@
 ClassEmbedder    — ldm/modules/encoders/modules.py:21-33 (`embedding.weight`), the cin256-v2 conditioning (1001 classes, 1000 = unconditional).
 LatentDiffusion  — a thin container of what the loop uses of ldm/models/diffusion/ddpm.py's LatentDiffusion: `model.diffusion_model` (the
                    UNetModel of ldm.py), `cond_stage_model`, the schedule buffers, get_learned_conditioning / apply_model / get_loss_at_t,
-                   and load_state_dict of a Lightning checkpoint's `state_dict`.  Not a Lightning module; no first stage, no EMA.
+                   and load_state_dict of a Lightning checkpoint's `state_dict`.  Not a Lightning module; no EMA; the
+                   decode side of the VQ first stage (`first_stage_model`, decode_first_stage) when built with first_stage_config.
 DDIMSampler      — ldm/models/diffusion/ddim.py: the same `sample(...)` call and results.  The whole S-step sample is ONE CUDA graph: per
                    step a fill of the timestep, the no-grad plan's forward at batch 2B (unconditional | conditional), and dp_ddim_cfg_step,
                    which forms the guided eps, writes x_prev and feeds both halves of the next forward's input.
 LDMPruneScorer   — the loop itself: classes -> guided DDIM-20 sample -> get_loss_at_t at t = iteration on the samples with fresh noise ->
                    the stop rule of --pruner diff-pruning / diff0 -> backward into the UNet's gradient arena.
+sample_for_fid   — sample_for_FID.py's render-and-score loop: guided DDIM samples, decode_first_stage on the engine (autoencoder.py), the
+                   save_image bytes on the device, FID moments of those bytes and / or the PNG files.
 
 Gradients reach the UNet only: the reference's trainable ClassEmbedder also gets a gradient from loss.backward(), but the pruner looks at
 `diffusion_model` alone, and the context enters the engine as a constant input.
 """
 from __future__ import annotations
 
+import os
 import random
+from contextlib import contextmanager
 from types import SimpleNamespace
 from typing import Callable, Dict, List, Optional, Sequence
 
@@ -24,6 +29,7 @@ import torch
 import torch.nn as nn
 
 from . import _lib as L
+from .autoencoder import VQModelInterface
 from .engine import _stream, frozen_weights, get_plan
 from .ldm import CIN256_V2_CONFIG, UNetModel
 from .scoring import TaylorScorer
@@ -109,9 +115,15 @@ class LatentDiffusion(nn.Module):
     l_simple_weight 1, logvar 0, original_elbo_weight 0, linear schedule 0.0015..0.0195 over 1000 steps, class-label cross-attention)."""
 
     def __init__(self, unet_config: Optional[dict] = None, cond_stage_config: Optional[dict] = None, timesteps: int = 1000,
-                 linear_start: float = 0.0015, linear_end: float = 0.0195, cond_stage_key: str = "class_label"):
+                 linear_start: float = 0.0015, linear_end: float = 0.0195, cond_stage_key: str = "class_label",
+                 first_stage_config: Optional[dict] = None, scale_factor: float = 1.0):
+        """first_stage_config: VQModelInterface's parameters (autoencoder.VQ_F4_CONFIG for cin256-v2) to hold the decode side of the
+        first stage as `first_stage_model`; None (the default) leaves it out, as the latent-space loops need it not."""
         super().__init__()
         self.model = DiffusionWrapper(UNetModel(**(unet_config or CIN256_V2_CONFIG)))
+        self.scale_factor = scale_factor        # ddpm.py:456-457 (scale_by_std False: a plain attribute, not in the state dict)
+        if first_stage_config is not None:
+            self.first_stage_model = VQModelInterface(**first_stage_config).eval()
         self.cond_stage_model = ClassEmbedder(**(cond_stage_config or dict(embed_dim=512, n_classes=1001, key=cond_stage_key)))
         self.cond_stage_key = cond_stage_key
         self.parameterization = "eps"
@@ -130,11 +142,31 @@ class LatentDiffusion(nn.Module):
     def load_state_dict(self, state_dict, strict: bool = True):
         """A Lightning checkpoint's `state_dict` (prune_ldm.py:21-28): `model.diffusion_model.*`, `cond_stage_model.*` and the three
         schedule buffers are loaded; `first_stage_model.*` (the VQ-f4 autoencoder), `model_ema.*` and the schedule buffers this container
-        does not hold are ignored."""
+        does not hold are ignored.  With a first stage, its `quantize.*`, `post_quant_conv.*` and `decoder.*` load too (its encoder,
+        quant_conv and loss are not built)."""
         own = set(self.state_dict().keys())
-        keep = {k: v for k, v in state_dict.items()
-                if k.startswith(("model.diffusion_model.", "cond_stage_model.")) or (k in own and "." not in k)}
+        prefixes = ("model.diffusion_model.", "cond_stage_model.")
+        if hasattr(self, "first_stage_model"):
+            prefixes += tuple(f"first_stage_model.{m}." for m in ("quantize", "post_quant_conv", "decoder"))
+        keep = {k: v for k, v in state_dict.items() if k.startswith(prefixes) or (k in own and "." not in k)}
         return super().load_state_dict(keep, strict=strict)
+
+    @contextmanager
+    def ema_scope(self, context=None):
+        """ddpm.py:171-184 with use_ema False (cin256-v2): the weights in use are the weights."""
+        yield None
+
+    @torch.no_grad()
+    def decode_first_stage(self, z, predict_cids=False, force_not_quantize=False):
+        """ddpm.py:706-765 without the patch-wise path: z / scale_factor (fp32) -> first_stage_model.decode, on the engine."""
+        if predict_cids:
+            raise NotImplementedError("decode_first_stage(predict_cids=True)")
+        if hasattr(self, "split_input_params"):
+            raise NotImplementedError("patch-wise decoding (split_input_params)")
+        if not hasattr(self, "first_stage_model"):
+            raise RuntimeError("this LatentDiffusion was built without first_stage_config: it holds no decoder")
+        inv = float(torch.tensor(1. / self.scale_factor, dtype=torch.float32))   # the fp32 scalar of `1. / self.scale_factor * z`
+        return self.first_stage_model.decode(z, force_not_quantize=predict_cids or force_not_quantize, inv_scale=inv)
 
     def get_learned_conditioning(self, c):
         """ddpm.py get_learned_conditioning with the ClassEmbedder: {cond_stage_key: (B,) labels} -> (B, 1, embed_dim)."""
@@ -443,3 +475,69 @@ class LDMPruneScorer:
         finally:
             self.unet.train(was_training)
         return torch.tensor(losses, dtype=torch.float32)
+
+
+@torch.no_grad()
+def sample_for_fid(model: LatentDiffusion, classes: Sequence[int] = range(1000), ipc: int = 50, batch_size: int = 50, ddim_steps: int = 250,
+                   eta: float = 0., scale: float = 3.0, out_dir: Optional[str] = None, fid_dims: int = 2048, inception=None,
+                   generator: Optional[torch.Generator] = None, decode_batch: int = 8):
+    """sample_for_FID.py:67-100: uc once; then ipc // batch_size rounds over `classes`, each a guided DDIM sample of batch_size latents
+    (DDIMSampler, one graph), decode_first_stage in micro-batches of decode_batch (one graph each) and dp_decode_images, which writes
+    the bytes tvu.save_image(clamp((x + 1) / 2, 0, 1)) would put in the PNG.  With an Inception model (fid.InceptionV3) the FID moments
+    of those bytes accumulate on the device, batch by batch, as fid.calculate_activation_statistics would add the saved files batched
+    by batch_size; with out_dir the files `{class_label}_{img_id}.png` are written on the host (img_id counts over the whole run).
+    Returns (mu, sigma, n_files): mu / sigma None without an Inception model, n_files 0 without out_dir."""
+    if inception is None and out_dir is None:
+        raise ValueError("sample_for_fid needs an Inception model, an output directory, or both")
+    if not hasattr(model, "first_stage_model"):
+        raise RuntimeError("sample_for_fid decodes its samples: build the LatentDiffusion with first_stage_config")
+    if out_dir is not None:
+        os.makedirs(out_dir, exist_ok=True)
+    dev = model.device
+    lib = L.load()
+    fs = model.first_stage_model
+    cfg = model.model.diffusion_model.config
+    shape = [cfg.in_channels, cfg.image_size, cfg.image_size]
+    inv = float(torch.tensor(1. / model.scale_factor, dtype=torch.float32))
+    key = model.cond_stage_key
+    sampler = DDIMSampler(model)
+    mom = block = None
+    if inception is not None:
+        from . import fid
+        block = fid._block_of(inception, fid_dims)
+        mom = fid.Moments(fid_dims)
+    u8 = None
+    img_id = n_files = 0
+    saved_batch = fs.decode_batch
+    fs.decode_batch = decode_batch
+    try:
+        with model.ema_scope():
+            uc = model.get_learned_conditioning({key: torch.tensor(batch_size * [1000]).to(dev)})
+            for _ in range(ipc // batch_size):
+                for class_label in classes:
+                    c = model.get_learned_conditioning({key: torch.tensor(batch_size * [class_label]).to(dev)})
+                    samples, _ = sampler.sample(S=ddim_steps, conditioning=c, batch_size=batch_size, shape=shape, verbose=False,
+                                                unconditional_guidance_scale=scale, unconditional_conditioning=uc, eta=eta,
+                                                generator=generator)
+                    for s in range(0, batch_size, decode_batch):
+                        y = fs.decode_chunk(samples[s:s + decode_batch], inv_scale=inv).plan.y_out
+                        if u8 is None:
+                            u8 = torch.empty((batch_size, y.H, y.W, y.C), dtype=torch.uint8, device=dev)
+                        n = min(decode_batch, batch_size - s)
+                        L.check(lib.dp_decode_images(y.ptr, y.ld, n, y.C, y.H, y.W, u8[s:s + n].data_ptr(), None, _stream()),
+                                "decode_images")
+                    if mom is not None:
+                        plan = inception.plan(batch_size, "u8", u8.shape[1:3])
+                        plan.load(u8)
+                        plan.run()
+                        mom.add(plan.feat[block])
+                    if out_dir is not None:
+                        from PIL import Image
+                        for img in u8.cpu().numpy():
+                            Image.fromarray(img).save(os.path.join(out_dir, f"{class_label}_{img_id}.png"))
+                            img_id += 1
+                            n_files += 1
+    finally:
+        fs.decode_batch = saved_batch
+    mu, sigma = mom.finalize() if mom is not None else (None, None)
+    return mu, sigma, n_files

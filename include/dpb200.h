@@ -422,6 +422,25 @@ typedef struct dp_ssim_args {
  * size or format. */
 int dp_ssim(const dp_ssim_args* a, dp_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * LDM first stage on the evaluation path (vq.cu): LatentDiffusion.decode_first_stage -> VQModelInterface.decode
+ * (ldm/models/diffusion/ddpm.py:706-713, ldm/models/autoencoder.py:274-282) and sample_for_FID.py's clamp / save_image.
+ * ------------------------------------------------------------------------------------------------ */
+/* VectorQuantizer2.forward on the decode path.  z: fp32 NCHW [N][D][H][W] (the sampler's latent); every value is first multiplied by
+ * inv_scale in fp32 (1 / scale_factor).  With quantize, each pixel's nearest codebook row j (codebook: fp32 [n_embed][D]) is the argmin
+ * over j of the fp64 sum ((z_0 - e_j0)^2 + (z_1 - e_j1)^2) + ... taken in that order (differences and squares of fp32 values are exact in
+ * fp64), the lowest index winning a tie, and out receives z + (e_j - z) rounded in fp32 as the straight-through expression rounds it;
+ * without quantize (force_not_quantize) out receives z.  out: NHWC view [N][H][W] of pixel stride ld_out >= D (the decoder's padded
+ * input; pad channels are not written).  indices (nullable, quantize only): int64 [N][H][W].  D <= 8 (DP_ERR_UNSUPPORTED). */
+int dp_vq_quantize(const float* z, int32_t N, int32_t D, int32_t H, int32_t W, float inv_scale, const float* codebook, int32_t n_embed,
+                   int32_t quantize, float* out, int64_t ld_out, int64_t* indices, dp_stream_t stream);
+/* The decoded images y (NHWC view [N][H][W], pixel stride ld >= C, values about [-1, 1]) as sample_for_FID.py saves them:
+ * v = clamp((y + 1) / 2, 0, 1) (each operation rounded in fp32), written as fp32 NCHW [N][C][H][W] to f32_nchw and / or as
+ * torchvision's save_image bytes trunc(clamp(v * 255 + 0.5, 0, 255)) to u8_nhwc ([N][H][W][C], the pixels of the PNG file).  At least
+ * one of the two outputs must be given. */
+int dp_decode_images(const float* y, int64_t ld, int32_t N, int32_t C, int32_t H, int32_t W, uint8_t* u8_nhwc, float* f32_nchw,
+                     dp_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

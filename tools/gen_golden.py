@@ -16,6 +16,7 @@ Outputs (all small, committed):
     tests/golden/ddim_tiny.pt      DDIMPipeline samples (uniform/eta 0/10 steps, quad/eta 0.5/7 steps) on TINY
     tests/golden/fid_*             FID Inception fixtures (gen_fid): weight-file layout, features of seeded weights, Frechet cases
     tests/golden/ssim_ref.pt       SSIM fixtures (gen_ssim): uint8 image pairs and utils_image.py's per-channel / per-image SSIM
+    tests/golden/vq_decoder_tiny.pt  the LDM's VQ first-stage Decoder (small config and VQ-f4 at a 16 x 16 latent) and nearest-code choices
     tests/golden/ldm_ddim_tiny.pt  guided DDIM sampling of the tiny LDM by ldm_exp's DDIMSampler, every step, and one get_loss_at_t pass
 """
 import argparse
@@ -798,13 +799,48 @@ def gen_ssim():
     print("ssim_ref.pt", os.path.getsize(os.path.join(OUT, "ssim_ref.pt")))
 
 
+VQ_TINY_DDCONFIG = dict(double_z=False, z_channels=3, resolution=16, in_channels=3, out_ch=3, ch=64, ch_mult=(1, 2), num_res_blocks=1,
+                        attn_resolutions=(), dropout=0.0)
+
+
+def gen_vq_decoder():
+    """The LDM's VQ first-stage Decoder from the UNMODIFIED reference module (ldm_exp/ldm/modules/diffusionmodules/model.py, imported
+    through ref_shim.install_ldm): for a small config (2 levels, 64 channels, 8 x 8 latent) and the full cin256-v2 VQ-f4 ddconfig at a
+    16 x 16 latent (64 x 64 output, 256 attention tokens), the state-dict keys, the seed and digest of the seed-s weights (torch.manual_seed(s);
+    Decoder(**cfg)), two seeded latents and the reference outputs; plus the nearest-code choices of the cdist formula
+    (diffusers/models/vae.py:338) and of taming's VectorQuantizer2 formula as recalled (z^2 + e^2 - 2 z e^T; taming is not in the reference
+    tree) for a seeded latent against a seeded 8192 x 3 codebook."""
+    ref_shim.install_ldm()
+    from ldm.modules.diffusionmodules.model import Decoder as RefDecoder
+    from diff_pruning_b200.autoencoder import VQ_F4_CONFIG
+    from oracle import vq_oracle as vo
+    out = {"configs": {}}
+    for name, ddcfg, hw, seed in (("tiny", VQ_TINY_DDCONFIG, 8, 0), ("vq_f4", dict(VQ_F4_CONFIG["ddconfig"]), 16, 1)):
+        torch.manual_seed(seed)
+        dec = RefDecoder(**ddcfg).eval()
+        sd = dec.state_dict()
+        g = torch.Generator().manual_seed(100 + seed)
+        z = torch.randn(2, ddcfg["z_channels"], hw, hw, generator=g)
+        with torch.no_grad():
+            y = dec(z)
+        out["configs"][name] = {"ddconfig": ddcfg, "seed": seed, "sd_keys": list(sd.keys()), "digest": vo.state_dict_digest(sd),
+                                "z": z, "out": y.detach()}
+        print("vq_decoder", name, tuple(y.shape), float(y.abs().max()))
+    g = torch.Generator().manual_seed(7)
+    code = (torch.rand(8192, 3, generator=g) * 2 - 1) / 8192 * 64
+    z = torch.randn(4096, 3, generator=g) * 0.004
+    out["codes"] = {"codebook_seed": 7, "z": z, "cdist": vo.nearest_code_cdist(z, code), "taming": vo.nearest_code_taming(z, code)}
+    torch.save(out, os.path.join(OUT, "vq_decoder_tiny.pt"))
+    print("vq_decoder_tiny.pt", os.path.getsize(os.path.join(OUT, "vq_decoder_tiny.pt")))
+
+
 if __name__ == "__main__":
     ap = argparse.ArgumentParser()
     ap.add_argument("--skip-cfg1", action="store_true")
     ap.add_argument("--only", default=None)
     a = ap.parse_args()
     torch.set_num_threads(os.cpu_count())
-    jobs = {"ssim": gen_ssim, "fid": gen_fid,"ldm_tiny": gen_ldm_tiny, "ldm_ddim": gen_ldm_ddim, "exp_importance": gen_exp_importance, "ref_pickle": gen_ref_pickle, "lsun_struct": gen_lsun_struct, "lr": gen_lr, "ckpt": gen_ckpt, "ddim": gen_ddim, "tiny": gen_tiny, "blocks": gen_blocks, "finetune": gen_finetune, "cifar_fwd": gen_cifar_fwd,
+    jobs = {"vq_decoder": gen_vq_decoder, "ssim": gen_ssim, "fid": gen_fid,"ldm_tiny": gen_ldm_tiny, "ldm_ddim": gen_ldm_ddim, "exp_importance": gen_exp_importance, "ref_pickle": gen_ref_pickle, "lsun_struct": gen_lsun_struct, "lr": gen_lr, "ckpt": gen_ckpt, "ddim": gen_ddim, "tiny": gen_tiny, "blocks": gen_blocks, "finetune": gen_finetune, "cifar_fwd": gen_cifar_fwd,
             "cfg1_s3": gen_cfg1_s3, "cfg3_s3": gen_cfg3_s3, "cfg1": gen_cfg1}
     for name, fn in jobs.items():
         if a.only and name != a.only:
