@@ -221,7 +221,9 @@ __global__ void copy_rows_kernel(const float* __restrict__ a, long long lda, flo
     y[r * ldy + c] = a[r * lda + c];
   }
 }
-__global__ void softmax_fwd_kernel(const float* __restrict__ s, float* __restrict__ p, long long rows, int cols) {
+// s and p may be one buffer (the engine normalises the attention scores in place): no __restrict__, so the loads stay coherent
+// (LDG.E, not ld.global.nc), and lane j reads in[j] before it writes out[j] of its own row
+__global__ void softmax_fwd_kernel(const float* s, float* p, long long rows, int cols) {
   long long row = blockIdx.x * (long long)(NT / 32) + (threadIdx.x >> 5);
   if (row >= rows) return;
   int lane = threadIdx.x & 31;
@@ -236,7 +238,9 @@ __global__ void softmax_fwd_kernel(const float* __restrict__ s, float* __restric
   float inv = 1.0f / sum;
   for (int j = lane; j < cols; j += 32) out[j] = expf(in[j] - mx) * inv;
 }
-__global__ void softmax_bwd_kernel(const float* __restrict__ p, const float* __restrict__ dp, float* __restrict__ ds, long long rows, int cols,
+// dp and ds may be one buffer (in place, as the engine runs it): no operand is __restrict__, so every load stays coherent; lane j reads dr[j]
+// in both passes before it writes o[j]
+__global__ void softmax_bwd_kernel(const float* p, const float* dp, float* ds, long long rows, int cols,
                                    uint32_t* __restrict__ amax_ds) {
   __shared__ float wmax[NT / 32];
   const long long row = blockIdx.x * (long long)(NT / 32) + (threadIdx.x >> 5);

@@ -205,7 +205,7 @@ class Plan:
         self._slot_tags: List[str] = []
         self._fslot: Dict[int, int] = {}
         self._fslot_bad: set = set()
-        self._bslot: Dict[int, dict] = {}
+        self._bslot: Dict[Tuple[int, int, int], dict] = {}
         one = torch.tensor([1.0], dtype=torch.float32).view(torch.int32).to(self.dev)
         self._wslots[AMAX_SLOTS - 1:] = one            # constant slot: bound 1.0 (softmax probabilities)
         self._one_slot = self._wslots.data_ptr() + 4 * (AMAX_SLOTS - 1)
@@ -404,12 +404,21 @@ class Plan:
         return slot
 
     def _dy_slot(self, steps: List[Step], v: View) -> int:
-        """Consumer side (backward): slot of max|v.grad|.  The writers of v.grad are built later; _finalize_build hands them the slot and
-        drops the dp_amax launch recorded here when every one of them can report its own maximum."""
+        """Consumer side (backward): slot of max|v.grad| over v's channel range.  The writers of v.grad are built later; _finalize_build
+        hands the slot to the writers that leave v.grad's final values and drops the dp_amax launch recorded here when they can all report
+        their own maximum.  One slot per view, not per buffer: the h half and the skip half of a concat buffer's gradient are read at
+        different points of the backward, and a commit into the h half's slot by a skip-half writer would race with the h half's
+        side-stream weight gradient reading it (tests/test_stream_races_gpu.py)."""
         g = self.gradof(v)
-        rec = self._bslot.get(v.t.data_ptr())
+        key = (v.t.data_ptr(), v.off, v.C)
+        rec = self._bslot.get(key)
         if rec is None:
-            rec = self._bslot[v.t.data_ptr()] = {"slot": self._new_slot(f"grad {v.N}x{v.H}x{v.W}x{v.t.shape[-1]}"), "flags": []}
+            rec = self._bslot[key] = {"slot": self._new_slot(f"grad {v.N}x{v.H}x{v.W}x{v.t.shape[-1]}[{v.off}:{v.off + v.C}]"),
+                                      "flags": [], "lists": []}
+        # one consumer per view and backward item: items run in reverse of their recording, the steps of one item in recorded order, so
+        # the last recorded consumer is the first to run only while no item records two (_finalize_build relies on it)
+        assert not any(l is steps for l in rec["lists"]), "two consumers of one gradient view in one backward item"
+        rec["lists"].append(steps)
         slot, flag, lib = rec["slot"], [True], self.lib
         rec["flags"].append(flag)
 
@@ -1205,18 +1214,37 @@ class Plan:
                 for view, setter, _ in it.writes:
                     setter(self.g_is_init(view))
                     self.g_mark(view)
-            # gradient amax slots: when every writer of a tensor's gradient reports its own maximum, the consumers' dp_amax launches go
-            writers: Dict[int, list] = {}
-            for it in self.bwd:
-                for view, _, amax_setter in it.writes:
-                    writers.setdefault(view.t.data_ptr(), []).append(amax_setter)
-            for key, rec in self._bslot.items():
-                ws = writers.get(key, [])
-                if ws and all(w is not None for w in ws):
-                    for w in ws:
-                        w(rec["slot"])
-                    for flag in rec["flags"]:
+            # gradient amax slots: the final values of a read view's gradient are left by its last writers (in execution order, the
+            # writers that are the last to touch some of its channels).  When they all report their own maximum, they commit into the
+            # view's slot and the consumers' dp_amax launches go.  Every other writer commits nowhere, and a writer commits into one slot
+            # only: no launch can raise a slot after its consumers (some of them on the side stream) have read it
+            order = [(view, amax_setter) for it in reversed(self.bwd) for view, _, amax_setter in it.writes]
+            owner: Dict[int, int] = {}
+            for (tptr, off, c), rec in self._bslot.items():
+                need, final = [(off, off + c)], []
+                for view, amax_setter in reversed(order):
+                    if not need:
+                        break
+                    if view.t.data_ptr() != tptr:
+                        continue
+                    lo, hi = view.off, view.off + view.C
+                    rest = [iv for a, b in need for iv in ((a, min(b, lo)), (max(a, hi), b)) if iv[0] < iv[1]] \
+                        if any(a < hi and lo < b for a, b in need) else need
+                    if rest is not need:
+                        final.append(amax_setter)
+                    need = rest
+                if need or not final or any(w is None or owner.get(id(w), rec["slot"]) != rec["slot"] for w in final):
+                    # the consumers measure the view themselves: the first of them in execution order (the last recorded: one consumer per
+                    # backward item, asserted in _dy_slot) is enough, the view's gradient is final by then, and a second dp_amax would
+                    # commit into the slot after a side-stream consumer of the first one has read it
+                    for flag in rec["flags"][:-1]:
                         flag[0] = False
+                    continue
+                for w in final:
+                    owner[id(w)] = rec["slot"]
+                    w(rec["slot"])
+                for flag in rec["flags"]:
+                    flag[0] = False
         self._packed_version = None
         if self._n_slots:       # every activation / gradient amax slot starts the pass at zero
             zero: List[Step] = []

@@ -217,6 +217,47 @@ def argkinds(name: str):
     return kinds
 
 
+_SINKS: list = []      # on_call of every active wrap_launches block, innermost last
+
+
+class wrap_launches:
+    """`with wrap_launches(lib, on_call):` every kernel-launching entry point of the library (the ones taking a stream last) calls
+    on_call(name, args, stream) before it runs: args are the arguments without the stream, struct arguments copied as they are at the
+    call.  Plans bind struct launches when they record them, so a plan must be built inside such a block; the wrappers it binds report
+    to whichever blocks are active when it runs, so a plan built in one block is seen by a later one."""
+
+    def __init__(self, lib, on_call):
+        self.lib, self.on_call, self.orig = lib, on_call, {}
+
+    def __enter__(self):
+        from diff_pruning_b200 import _lib as L
+        from diff_pruning_b200.engine import _copy_args
+        _SINKS.append(self.on_call)
+        for name, (_, argtypes) in L._SIGS.items():
+            if not argtypes or argtypes[-1] is not C.c_void_p:      # launches take the stream last; the rest are host queries
+                continue
+            fn, kinds = getattr(self.lib, name), argkinds(name)
+            if getattr(fn, "_dp_wrapped", False):                  # an outer block wrapped it already
+                continue
+
+            def wrapped(*args, fn=fn, kinds=kinds, name=name):
+                if _SINKS:
+                    snap = [_copy_args(getattr(v, "_obj", v)) if k == "s" else v for k, v in zip(kinds, args[:-1])]
+                    for sink in list(_SINKS):
+                        sink(name, snap, args[-1])
+                return fn(*args)
+            wrapped._dp_wrapped = True
+            self.orig[name] = fn
+            setattr(self.lib, name, wrapped)
+        return self
+
+    def __exit__(self, *exc):
+        _SINKS.remove(self.on_call)
+        for name, fn in self.orig.items():
+            setattr(self.lib, name, fn)
+        return False
+
+
 def _ptr_key(v, esz: int = 4):
     """A pointer's part of the key: NULL or not, and its 16-byte alignment phase in elements of `esz` bytes (the element offset of a
     view mod 16 / esz)."""

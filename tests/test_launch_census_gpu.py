@@ -43,27 +43,12 @@ def S():
 
 # ---------------------------------------------------------------------------------------------------------------------- capture
 def _capture(lib, run):
-    """Calls every kernel-launching entry point receives while run() builds a fresh plan and makes one eager pass: [(name, args)]."""
-    from diff_pruning_b200 import _lib as L
-    from diff_pruning_b200.engine import _copy_args
-    calls, orig = [], {}
-    for name, (_, argtypes) in L._SIGS.items():
-        if not argtypes or argtypes[-1] is not C.c_void_p:      # launches take the stream last; the rest are host queries
-            continue
-        fn, kinds = getattr(lib, name), lc.argkinds(name)
-
-        def wrapped(*args, fn=fn, kinds=kinds, name=name):
-            snap = [_copy_args(getattr(v, "_obj", v)) if k == "s" else v for k, v in zip(kinds, args[:-1])]
-            calls.append((name, snap))
-            return fn(*args)
-        orig[name] = fn
-        setattr(lib, name, wrapped)
-    try:
+    """Calls every kernel-launching entry point receives while run() builds a fresh plan and makes one eager pass: [(name, args)]
+    (the stream each call was enqueued on is dropped: the census replays launches one at a time)."""
+    calls = []
+    with lc.wrap_launches(lib, lambda name, args, stream: calls.append((name, args))):
         run()
         torch.cuda.synchronize()
-    finally:
-        for name, fn in orig.items():
-            setattr(lib, name, fn)
     return calls
 
 
