@@ -768,7 +768,6 @@ static int gn_validate(const dp_gn_args* a) {
   DP_REQUIRE(a && a->x && a->gamma && a->beta && a->mean && a->rstd && a->workspace, DP_ERR_NULL);
   DP_REQUIRE(a->N > 0 && a->HW > 0 && a->C > 0 && a->G > 0 && a->C % a->G == 0, DP_ERR_SHAPE);
   DP_REQUIRE((a->C <= NT * MAXCPT || ln_fast(a)) && a->G <= 1024, DP_ERR_UNSUPPORTED);
-  DP_REQUIRE(a->N <= 65535, DP_ERR_SHAPE);
   DP_REQUIRE(a->ldx >= a->C, DP_ERR_SHAPE);
   DP_REQUIRE(a->dropout_p >= 0.f && a->dropout_p < 1.f, DP_ERR_SHAPE);
   return DP_OK;
@@ -786,6 +785,9 @@ extern "C" int dp_groupnorm_fwd(const dp_gn_args* a, dp_stream_t stream) {
     ln_fwd_kernel<<<(unsigned)((a->N + 7) / 8), 256, 0, st>>>(*a);
     return dp_check_launch();
   }
+  // the GroupNorm kernels take one image per grid row; the row kernels above take any N (the LDM transformer's LayerNorm runs over
+  // every token of the batch: 100 x 1024 rows at the 32 x 32 level of a batch-100 guided sample)
+  DP_REQUIRE(a->N <= 65535, DP_ERR_SHAPE);
   Map mp = v4 ? make_map4(a->HW, a->C) : make_map(a->HW, a->C);
   dim3 grid(mp.nchunks, a->N);
   if (v4) {
@@ -817,6 +819,7 @@ extern "C" int dp_groupnorm_bwd(const dp_gn_args* a, dp_stream_t stream) {
                   al16(a->dx_add, a->ldadd) && al16(a->dx_add2, a->ldadd2);
   DP_REQUIRE(!(a->fin && ln_fast(a)), DP_ERR_UNSUPPORTED);     // the row kernels take dgamma / dbeta from x and dy, not from fin
   if (v4 && ln_fast(a) && al16(a->gamma, 0)) {      // LayerNorm over tokens: row kernel for dx, chunked column sums for dgamma / dbeta
+    DP_REQUIRE((a->N + LN_ROWS - 1) / LN_ROWS <= 65535, DP_ERR_SHAPE);     // one grid row per chunk of the column sums
     ln_bwd_dx_kernel<<<(unsigned)((a->N + 7) / 8), 256, 0, st>>>(*a);
     if ((rc = dp_check_launch())) return rc;
     if (a->dgamma || a->dbeta) {
@@ -828,6 +831,7 @@ extern "C" int dp_groupnorm_bwd(const dp_gn_args* a, dp_stream_t stream) {
     }
     return rc;
   }
+  DP_REQUIRE(a->N <= 65535, DP_ERR_SHAPE);          // one image per grid row
   Map mp = v4 ? make_map4(a->HW, a->C) : make_map(a->HW, a->C);
   char* ws = (char*)a->workspace;
   float* part = (float*)ws;

@@ -76,13 +76,18 @@ def splitk_count(need_floats: int, rows: int, cols: int, stages: int) -> int:
     return max(1, min(ks, 16, stages // 4))
 
 
+MAX_SPLIT_STAGES = 147     # conv_tc.cu PS_MAX_SPLIT_STAGES: 4 x 147 = 588 accumulator updates per split, within L_MAX with 16 splits
+
+
 def pick_ksplit(tiles: int, iters: int, num_sms: int):
     """conv_tc.cu's pick_ksplit: (K splits, pipeline stages per split) of a persistent-kernel launch with `tiles` output tiles of `iters`
-    stages each.  No split when the tiles already cover half the SMs or there are fewer than 8 stages; otherwise enough work items to
-    fill the SMs, at least 4 stages per split, at most 16 splits, and no empty split."""
-    if tiles * 2 > num_sms or iters < 8:
-        return 1, iters
-    ks = min(num_sms // tiles, iters // 4, 16)
+    stages each.  To fill the SMs: no split when the tiles already cover half the SMs or there are fewer than 8 stages, otherwise enough
+    work items to fill them, at least 4 stages per split, at most 16 splits.  Whatever the tiles, at least ceil(iters / MAX_SPLIT_STAGES)
+    splits, so that no chain is longer than MAX_SPLIT_STAGES stages; and no empty split."""
+    ks = 1
+    if tiles * 2 <= num_sms and iters >= 8:
+        ks = min(num_sms // tiles, iters // 4, 16)
+    ks = max(ks, -(-iters // MAX_SPLIT_STAGES))
     if ks < 2:
         return 1, iters
     ips = -(-iters // ks)
@@ -187,6 +192,24 @@ def ddim_step_ref(x, e, nz, sb: float, sa: float, clip: float, sap: float, dirc:
         ref = ref + sigma * nz.double()
         mag = mag + sigma * nz.double().abs()
     return ref, sap * ex0 + 4 * U * mag
+
+
+def softmax_fwd_bound(ref, z, cols):
+    """Element-wise bound of dp_softmax_fwd (one warp per row: z = x - max in fp32, e = expf(z), per-lane sums of ceil(cols / 32)
+    e's, a 5-level butterfly over the lanes, p = e * (1 / sum)), relative to p:
+      * its own exponential: expf is within 2 ulp (2^-22 relative), and the fp32 rounding of z moves exp(z) by up to 2^-24 |z|;
+      * the row sum: the same exponential errors weighted by the terms, 2^-22 + 2^-24 sum_k p_k |z_k|, and the fixed-order rounding
+        of the sum.  Every partial sum is at most the row sum S (the terms are positive) and one lane's chain is ceil(cols / 32)
+        additions plus the 5 butterfly levels: sum_bound's model with S for s, (SUM_ALPHA + 8 sqrt(n)) 2^-24 (the lane holding the
+        row's largest term adds its other terms to a partial of about S from the start, so its n roundings are each of order 2^-24 S);
+      * the reciprocal and the product: one rounding each.
+    The argument terms are doubled for room; values below 2^-126 are held to 2^-126 absolute (subnormal exponentials).  An emulation
+    of the kernel's order of operations in torch fp32 on an H100 is bit-identical to it; at 2 x 32768 rows of 4096 (the VQ-f4 attention
+    at batch 8) its worst row-sum error is 17.4 2^-24, its worst element 35 2^-24, against a bound of 108 2^-24 and more."""
+    n = -(-cols // 32) + 5
+    rel = (2.0 ** -22 + 2.0 ** -23 * z.abs()) + (2.0 ** -22 + 2.0 ** -23 * (ref * z.abs()).sum(-1, keepdim=True))
+    rel = rel + (SUM_ALPHA + 8.0 * math.sqrt(n)) * U + 2 * U
+    return rel * ref + 2.0 ** -126
 
 
 def violations(got: torch.Tensor, ref: torch.Tensor, bound: torch.Tensor, limit: int = 8):

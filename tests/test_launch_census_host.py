@@ -154,15 +154,21 @@ def _inception_convs():
 
 def test_general_split_count_follows_the_kernel_rule():
     """launch_census.general_split restates conv_tc.cu's pick_ksplit over the general-geometry kernel's tiles and stages: hand-computed
-    cases (splits only where the tiles cover less than half of 132 SMs, capped at 16, at least 4 stages per split, no empty split),
-    and on every Inception convolution at batches 50, 128 and 256 the rule's invariants hold and the chain stays within L_MAX."""
+    cases (splits to fill the SMs only where the tiles cover less than half of 132 SMs, capped at 16, at least 4 stages per split; at
+    least enough splits that none walks more than MAX_SPLIT_STAGES stages, so that even 16 of them keep the chain within L_MAX; no empty
+    split), and on every Inception convolution at batches 50, 128 and 256 the rule's invariants hold and the chain stays within L_MAX."""
     sms = 132
+    assert lc.chain_general(16, lc.MAX_SPLIT_STAGES) <= lc.L_MAX
     assert lc.pick_ksplit(1, 100, sms) == (15, 7)        # 16 splits of 7 stages would leave the last one empty
     assert lc.pick_ksplit(4, 9, sms) == (2, 5)
     assert lc.pick_ksplit(66, 8, sms) == (2, 4)
     assert lc.pick_ksplit(67, 100, sms) == (1, 100)      # tiles cover more than half the SMs
     assert lc.pick_ksplit(1, 7, sms) == (1, 7)           # fewer than 8 stages
     assert lc.pick_ksplit(40, 11, sms) == (2, 6)         # 3 SMs per tile, but at least 4 stages per split: 2 splits of 6
+    assert lc.pick_ksplit(120, 216, sms) == (2, 108)     # tiles fill the SMs, but 216 stages are longer than one split may walk
+    assert lc.pick_ksplit(400, 270, sms) == (2, 135)
+    assert lc.pick_ksplit(400, 147, sms) == (1, 147)     # the longest chain that stays whole
+    assert lc.pick_ksplit(1, 300, sms) == (16, 19)       # the SM rule already splits further than the chain rule
     convs = _inception_convs()
     assert len(convs) == 94
     geo = {c[:9]: c for c in convs}
@@ -317,3 +323,35 @@ def test_global_mean_bound_rejects_a_running_fp32_sum():
         acc = acc + flat[:, :, k]
     run32 = acc / 73 / 73
     _affected_majority((run32.double() - ref).abs() > bound, torch.ones_like(ref, dtype=torch.bool), "running fp32 sum over 73 x 73")
+
+
+def _emulate_softmax_fp32(x: torch.Tensor, lanes_summed: int = 32, dtype=torch.float32) -> torch.Tensor:
+    """softmax_fwd_kernel on the host: fp32 z = x - max, exp, per-lane sums of every 32nd term in `dtype`, a butterfly over the first
+    `lanes_summed` lanes, p = e * (1 / sum)."""
+    rows, cols = x.shape
+    z = x - x.amax(-1, keepdim=True)
+    e = torch.exp(z)
+    acc = torch.zeros(rows, 32, dtype=dtype)
+    for k in range(cols // 32):
+        acc = acc + e[:, 32 * k:32 * k + 32].to(dtype)
+    acc = acc.float()[:, :lanes_summed]
+    o = lanes_summed // 2
+    while o:
+        acc = acc + acc[:, torch.arange(lanes_summed) ^ o]
+        o //= 2
+    return e * (1.0 / acc[:, :1])
+
+
+def test_softmax_bound_admits_the_kernel_order_and_rejects_a_lost_lane_or_a_half_precision_sum():
+    """softmax_fwd_bound at the 4096 columns of the VQ-f4 attention: the kernel's own order of operations in fp32 stays within it, while
+    a butterfly that drops half the lanes, or lane sums kept in fp16, violate it on most rows."""
+    x = torch.randn(256, 4096, generator=torch.Generator().manual_seed(5)) * 3
+    ref = torch.softmax(x.double(), -1)
+    bound = lc.softmax_fwd_bound(ref, x.double() - x.double().amax(-1, keepdim=True), 4096)
+    worst, where = lc.violations(_emulate_softmax_fp32(x), ref, bound)
+    assert not where and worst < 0.5, worst
+    for what, got in (("16 lanes", _emulate_softmax_fp32(x, 16)), ("fp16 lane sums", _emulate_softmax_fp32(x, dtype=torch.float16))):
+        bad = ((got.double() - ref).abs() > bound).any(-1).double().mean()
+        print(f"{what}: violates the bound on {float(bad):.1%} of the rows")
+        assert float(bad) > 0.5, what
+    print(f"kernel order: worst err/bound {worst:.3f}")

@@ -124,26 +124,32 @@ def test_ddim_cfg_step_census(lib):
                       unconditional_guidance_scale=scale, unconditional_conditioning=uc, generator=torch.Generator().manual_seed(3))
     calls = [(n, a) for n, a in _capture(lib, run) if n == "dp_ddim_cfg_step"]
     assert len(calls) == 8
-    seen, worst = {}, 0.0
+    seen, rep = {}, {}
     for name, args in calls:
         seen.setdefault(lc.launch_key(name, lc.argkinds(name), args), args)
     g = torch.Generator().manual_seed(17)
     for args in seen.values():
-        _, ld_eps, _, nzp, _, _, ld_in, _, B, C_, H, W, guided, scale, sb, sa, sap, dirc, sig = args
-        x = torch.randn(B, C_, H, W, generator=g).cuda() * 4
-        e_all = torch.randn((2 if guided else 1) * B, C_, H, W, generator=g).cuda()
-        nz = torch.randn(B, C_, H, W, generator=g).cuda() if nzp else None
-        out, _, x0 = _run_kernel_raw(lib, e_all, x, nz, ld_eps, ld_in, guided, scale, (sb, sa, sap, dirc, sig))
-        e = e_all[:B] + scale * (e_all[B:] - e_all[:B]) if guided else e_all[:B]
-        k = [torch.full((B, 1, 1, 1), v, device="cuda") for v in (sb, sa, sap, dirc, sig)]
-        want_x0 = (x - k[0] * e) / k[1]
-        want = k[2] * want_x0 + k[3] * e + (k[4] * nz if nz is not None else 0.)
-        assert torch.equal(x0, want_x0) and torch.equal(out, want), "dp_ddim_cfg_step is not bit-exact"
-        r64, bound = lc.ddim_step_ref(x, e, nz, sb, sa, 0.0, sap, dirc, sig)
-        w, where = lc.violations(out, r64, bound)
-        assert not where, where
-        worst = max(worst, w)
-    print(f"\ndp_ddim_cfg_step census: {len(calls)} launches, {len(seen)} distinct, worst err/bound {worst:.3g}")
+        replay_ddim_cfg_step(lib, g, "dp_ddim_cfg_step", args, rep)
+    print(f"\ndp_ddim_cfg_step census: {len(calls)} launches, {len(seen)} distinct, worst err/bound {max(rep['dp_ddim_cfg_step']):.3g}")
+
+
+def replay_ddim_cfg_step(lib, g, name, args, rep):
+    """One captured dp_ddim_cfg_step launch replayed on fresh seeded buffers at its geometry, pitches and fp32 coefficients: bit-exact
+    against the torch fp32 restatement, and within launch_census.ddim_step_ref's fp64 bound (err / bound appended to rep[name])."""
+    _, ld_eps, _, nzp, _, _, ld_in, _, B, C_, H, W, guided, scale, sb, sa, sap, dirc, sig = args
+    x = torch.randn(B, C_, H, W, generator=g).cuda() * 4
+    e_all = torch.randn((2 if guided else 1) * B, C_, H, W, generator=g).cuda()
+    nz = torch.randn(B, C_, H, W, generator=g).cuda() if nzp else None
+    out, _, x0 = _run_kernel_raw(lib, e_all, x, nz, ld_eps, ld_in, guided, scale, (sb, sa, sap, dirc, sig))
+    e = e_all[:B] + scale * (e_all[B:] - e_all[:B]) if guided else e_all[:B]
+    k = [torch.full((B, 1, 1, 1), v, device="cuda") for v in (sb, sa, sap, dirc, sig)]
+    want_x0 = (x - k[0] * e) / k[1]
+    want = k[2] * want_x0 + k[3] * e + (k[4] * nz if nz is not None else 0.)
+    assert torch.equal(x0, want_x0) and torch.equal(out, want), "dp_ddim_cfg_step is not bit-exact"
+    r64, bound = lc.ddim_step_ref(x, e, nz, sb, sa, 0.0, sap, dirc, sig)
+    w, where = lc.violations(out, r64, bound)
+    assert not where, where
+    rep.setdefault(name, []).append(w)
 
 
 def _run_kernel_raw(lib, e_all, x, nz, ld_eps, ld_in, guided, scale, k):
