@@ -23,22 +23,26 @@ static inline Map make_map(int HW, int C) {
 // Dropout keep-mask: a counter-based hash (splitmix64) of (seed, element index / 4) yields 64 bits = one 16-bit uniform for each of
 // 4 consecutive elements (the float4 kernels hash once per load); keep if u16 >= thr = round(p * 65536), survivors scaled by
 // 65536 / (65536 - thr) (the exact inverse keep rate).  Forward and backward regenerate the same mask from the element index alone.
+// The combined seed goes through the splitmix64 finalizer once before the counter is added: the counter steps the state by the golden
+// ratio constant, so unmixed seeds that differ by k times that constant (the engine's k-th dropout layer) drew masks shifted by 4k elements.
 struct Drop {
   uint64_t seed; uint32_t thr; float inv; bool on;
 };
+__device__ __forceinline__ uint64_t mix64(uint64_t z) {
+  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+  return z ^ (z >> 31);
+}
 __device__ __forceinline__ Drop make_drop(const dp_gn_args& a) {
   Drop d;
   d.on = a.dropout_p > 0.f;
-  d.seed = a.dropout_seed + ((d.on && a.dropout_seed_dev) ? *a.dropout_seed_dev : 0ull);
+  d.seed = mix64(a.dropout_seed + ((d.on && a.dropout_seed_dev) ? *a.dropout_seed_dev : 0ull));
   d.thr = d.on ? __float2uint_rn(a.dropout_p * 65536.f) : 0u;
   d.inv = 65536.f / (float)(65536u - d.thr);
   return d;
 }
 __device__ __forceinline__ uint64_t drop_bits(uint64_t seed, uint64_t group) {
-  uint64_t z = seed + 0x9E3779B97F4A7C15ull * (group + 1);
-  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
-  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
-  return z ^ (z >> 31);
+  return mix64(seed + 0x9E3779B97F4A7C15ull * (group + 1));
 }
 __device__ __forceinline__ float keep_scale(const Drop& d, uint64_t idx) {
   const uint32_t u = (uint32_t)(drop_bits(d.seed, idx >> 2) >> (16 * (int)(idx & 3))) & 0xFFFFu;
@@ -189,6 +193,8 @@ __global__ void __launch_bounds__(NT) gn_apply_kernel(const dp_gn_args a, const 
 }
 
 // ---- backward ----
+// The backward applies the keep-scale to dy with __fmul_rn, which is never contracted into a following FMA: with dropout the backward is
+// bit for bit the p = 0 backward of dy * mask.
 __device__ __forceinline__ float gn_dy(const dp_gn_args& a, float g, float y) {   // g: dy with the dropout keep-scale already applied
   if (a.silu) { float s = sigmoidf_fast(y); g *= s * (1.f + y * (1.f - s)); }
   return g;
@@ -218,7 +224,7 @@ __global__ void __launch_bounds__(NT) gn_bwd_partial_kernel(const dp_gn_args a, 
         float xh = (__ldg(xb + (long long)pix * a.ldx + c) - mu[u]) * rs[u];
         float y = fmaf(xh, ga[u], be[u]);
         float g = __ldg(db + (long long)pix * a.lddy + c);
-        if (drop.on) g *= keep_scale(drop, ((uint64_t)n * a.HW + pix) * a.C + c);
+        if (drop.on) g = __fmul_rn(g, keep_scale(drop, ((uint64_t)n * a.HW + pix) * a.C + c));
         g = gn_dy(a, g, y);
         s1[u] += g; s2[u] += g * xh;
       }
@@ -346,7 +352,7 @@ __global__ void __launch_bounds__(NT) gn_bwd_apply_kernel(const dp_gn_args a, co
         float xh = (__ldg(xb + (long long)pix * a.ldx + c) - mu[u]) * rs[u];
         float y = fmaf(xh, ga[u], be[u]);
         float g = __ldg(db + (long long)pix * a.lddy + c);
-        if (drop.on) g *= keep_scale(drop, ((uint64_t)n * a.HW + pix) * a.C + c);
+        if (drop.on) g = __fmul_rn(g, keep_scale(drop, ((uint64_t)n * a.HW + pix) * a.C + c));
         g = gn_dy(a, g, y);
         float d = rs[u] * (ga[u] * g - c1[u] - xh * c2[u]);
         if (ab) d += ab[(long long)pix * a.ldadd + c];
@@ -526,7 +532,7 @@ __global__ void __launch_bounds__(NT, 4) gn_bwd_partial4_kernel(const dp_gn_args
             float k[4];
             keep_scale4(drop, ((uint64_t)n * a.HW + pix) * a.C + c0, k);
 #pragma unroll
-            for (int e = 0; e < 4; ++e) ds[e] *= k[e];
+            for (int e = 0; e < 4; ++e) ds[e] = __fmul_rn(ds[e], k[e]);
           }
 #pragma unroll
           for (int e = 0; e < 4; ++e) {
@@ -599,7 +605,7 @@ __global__ void __launch_bounds__(NT, 4) gn_bwd_apply4_kernel(const dp_gn_args a
           float k[4];
           keep_scale4(drop, ((uint64_t)n * a.HW + pix) * a.C + c0, k);
 #pragma unroll
-          for (int e = 0; e < 4; ++e) ds[e] *= k[e];
+          for (int e = 0; e < 4; ++e) ds[e] = __fmul_rn(ds[e], k[e]);
         }
 #pragma unroll
         for (int e = 0; e < 4; ++e) {

@@ -835,7 +835,7 @@ class Plan:
             a.mean, a.rstd = stats.data_ptr(), stats.data_ptr() + 4 * x.N * gp
             if dropout_p > 0:
                 a.dropout_p = dropout_p
-                a.dropout_seed = (0x9E3779B97F4A7C15 * self._n_dropout + 0x632BE59BD9B4E019 * i) & 0xFFFFFFFFFFFFFFFF
+                a.dropout_seed = dropout_layer_seed(self._n_dropout, i)
                 a.dropout_seed_dev = self.dropout_seed_dev.data_ptr()
             self.scratch("gn_ws", (lib.dp_groupnorm_workspace_bytes(a.N, a.HW, a.C, a.G) + 3) // 4)
             self._late.append(lambda a=a: setattr(a, "workspace", self.sptr("gn_ws")))
@@ -1636,15 +1636,27 @@ def unet_apply(model, sample: torch.Tensor, timesteps: torch.Tensor, context: Op
     return plan.output_nchw()
 
 
-def _dropout_seed(step: int) -> int:
-    """Per-step dropout seed, decorrelated across data-parallel ranks (every rank must draw its own masks)."""
-    rank = 0
+def dropout_layer_seed(layer: int, part: int) -> int:
+    """dp_gn_args.dropout_seed of channel part `part` of the plan's `layer`-th dropout GroupNorm (counted from 1 in build order).  The
+    kernel adds the step / rank seed of the device scalar and mixes the sum, so these only have to differ between launches."""
+    return (0x9E3779B97F4A7C15 * layer + 0x632BE59BD9B4E019 * part) & 0xFFFFFFFFFFFFFFFF
+
+
+def _dist_rank() -> int:
     try:
         import torch.distributed as dist
         if dist.is_available() and dist.is_initialized():
-            rank = dist.get_rank()
+            return dist.get_rank()
     except Exception:
-        rank = 0
+        pass
+    return 0
+
+
+def _dropout_seed(step: int, rank: Optional[int] = None) -> int:
+    """Per-step dropout seed (the value of Plan.dropout_seed_dev), decorrelated across data-parallel ranks (every rank must draw its own
+    masks); `rank` defaults to this process's rank."""
+    if rank is None:
+        rank = _dist_rank()
     return (0x5DEECE66D * step + 0x9E3779B97F4A7C15 * rank) & 0x7FFFFFFFFFFF
 
 

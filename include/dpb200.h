@@ -235,7 +235,10 @@ typedef struct dp_gn_args {
   void* workspace;                /* dp_groupnorm_workspace_bytes() */
   /* dropout folded behind the SiLU (resnet.py:631): keep-mask from a counter-based hash of (seed, element index / 4), one 16-bit uniform
    * per element: keep iff u16 >= round(p * 65536), survivors scaled by 65536 / (65536 - round(p * 65536)); the backward regenerates
-   * the same mask from the element index ; p = 0 disables */
+   * the same mask from the element index ; p = 0 disables.  The element index is (n * HW + pixel) * C + c over the dense extent (never
+   * the pitch).  With s = dropout_seed + *dropout_seed_dev, m = fmix(s) and fmix the splitmix64 finalizer, the 64 bits of element group
+   * i = index / 4 are fmix(m + 0x9E3779B97F4A7C15 * (i + 1)), and element index reads bits [16 * (index % 4), +16).  Distinct seeds
+   * give unrelated masks (no seed is a shifted copy of another's stream) */
   float dropout_p; uint64_t dropout_seed;
   const uint64_t* dropout_seed_dev; /* optional DEVICE scalar added to dropout_seed (lets a captured CUDA graph
                                        draw a fresh mask every replay) */
