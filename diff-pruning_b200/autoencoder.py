@@ -1,14 +1,15 @@
-"""The VQ-f4 first stage of the class-conditional LDM, decode side only (cin256-v2.yaml first_stage_config: VQModelInterface, 8192 x 3
-codebook, Decoder ch 128, ch_mult (1, 2, 4), 2 res blocks, no attention resolutions).
+"""The VQ-f4 first stage of the class-conditional LDM (cin256-v2.yaml first_stage_config: VQModelInterface, 8192 x 3 codebook,
+Encoder / Decoder ch 128, ch_mult (1, 2, 4), 2 res blocks, no attention resolutions).
 
-Module tree, construction order and parameter names of the reference's `ldm/modules/diffusionmodules/model.py:38-214,462-568`
-(Normalize, Upsample, ResnetBlock, AttnBlock, Decoder) and of `ldm/models/autoencoder.py:14-43,264-282` (VQModel / VQModelInterface,
-with taming's VectorQuantizer2 holding `embedding`), so `torch.manual_seed(s); Decoder(**cfg)` reproduces the reference Decoder's
-parameters and a Lightning checkpoint's `first_stage_model.{quantize,post_quant_conv,decoder}.*` load as they are.  The encoder,
-quant_conv and the loss are not built.
+Module tree, construction order and parameter names of the reference's `ldm/modules/diffusionmodules/model.py:38-214,368-568`
+(Normalize, Upsample, Downsample, ResnetBlock, AttnBlock, Encoder, Decoder) and of `ldm/models/autoencoder.py:14-43,264-282` (VQModel /
+VQModelInterface, with taming's VectorQuantizer2 holding `embedding`), so `torch.manual_seed(s); Encoder(**cfg)` / `Decoder(**cfg)`
+reproduce the reference modules' parameters and a Lightning checkpoint's `first_stage_model.{encoder,decoder,quantize,quant_conv,
+post_quant_conv}.*` load as they are.  The encoder and quant_conv are built on request (with_encoder=True); the loss is not built.
 
-On CUDA, VQModelInterface.decode is the planned sm_90a engine (engine.Plan._build_vq_decoder) behind dp_vq_quantize, one CUDA graph per
-micro-batch of latents; under models.trace_mode() the modules run as torch ops (structure tests).  No CPU fallback otherwise.
+On CUDA, VQModelInterface.decode is the planned sm_90a engine (engine.Plan._build_vq_decoder) behind dp_vq_quantize, and encode the
+forward-only encoder plan (engine.Plan._build_vq_encoder), each one CUDA graph per micro-batch; under models.trace_mode() the modules run
+as torch ops (structure tests).  No CPU fallback otherwise.
 """
 from __future__ import annotations
 
@@ -30,6 +31,7 @@ VQ_F4_CONFIG = dict(  # ldm_exp/configs/latent-diffusion/cin256-v2.yaml first_st
                   attn_resolutions=(), dropout=0.0))
 
 DECODE_MICRO_BATCH = 8    # latents per decoder plan: about 1 GB of activations per 256 x 256 image, plus its 4096^2 attention matrix
+ENCODE_MICRO_BATCH = 8    # images per encoder plan
 
 
 def Normalize(in_channels, num_groups=32):
@@ -55,13 +57,28 @@ class Upsample(nn.Module):
         return self.conv(F.interpolate(x, scale_factor=2.0, mode="nearest"))
 
 
+class Downsample(nn.Module):
+    """model.py:60-79 (with_conv): F.pad(x, (0, 1, 0, 1)), then a 3x3 stride-2 convolution without padding."""
+
+    def __init__(self, in_channels, with_conv):
+        super().__init__()
+        if not with_conv:
+            raise NotImplementedError("resamp_with_conv=False")
+        self.with_conv = with_conv
+        self.conv = nn.Conv2d(in_channels, in_channels, kernel_size=3, stride=2, padding=0)
+
+    def forward(self, x):
+        return self.conv(F.pad(x, (0, 1, 0, 1), mode="constant", value=0))
+
+
 class ResnetBlock(nn.Module):
-    """model.py:82-141 as the decoder builds it: no time embedding (temb_channels 0), a 1x1 nin_shortcut when the width changes."""
+    """model.py:82-141 as the encoder and decoder build it: no time embedding (temb_channels 0), a 1x1 nin_shortcut when the width
+    changes."""
 
     def __init__(self, *, in_channels, out_channels=None, conv_shortcut=False, dropout, temb_channels=512):
         super().__init__()
         if temb_channels > 0 or conv_shortcut:
-            raise NotImplementedError("the decoder's ResnetBlock has no time embedding and a 1x1 shortcut")
+            raise NotImplementedError("the first stage's ResnetBlock has no time embedding and a 1x1 shortcut")
         self.in_channels = in_channels
         out_channels = in_channels if out_channels is None else out_channels
         self.out_channels = out_channels
@@ -103,6 +120,61 @@ class AttnBlock(nn.Module):
         w_ = F.softmax(w_, dim=2)
         h_ = torch.bmm(v.reshape(b, c, h * w), w_.permute(0, 2, 1)).reshape(b, c, h, w)
         return x + self.proj_out(h_)
+
+
+class Encoder(nn.Module):
+    """model.py:368-460 (attn_type "vanilla", double_z False)."""
+
+    def __init__(self, *, ch, out_ch, ch_mult=(1, 2, 4, 8), num_res_blocks, attn_resolutions, dropout=0.0, resamp_with_conv=True,
+                 in_channels, resolution, z_channels, double_z=True, use_linear_attn=False, attn_type="vanilla", **ignore_kwargs):
+        super().__init__()
+        if use_linear_attn or attn_type != "vanilla" or double_z:
+            raise NotImplementedError("only the vanilla-attention Encoder with double_z=False (the VQ-f4 first stage)")
+        self.ch, self.temb_ch = ch, 0
+        self.num_resolutions, self.num_res_blocks = len(ch_mult), num_res_blocks
+        self.resolution, self.in_channels = resolution, in_channels
+        self.conv_in = nn.Conv2d(in_channels, self.ch, kernel_size=3, stride=1, padding=1)
+        curr_res = resolution
+        in_ch_mult = (1,) + tuple(ch_mult)
+        self.in_ch_mult = in_ch_mult
+        self.down = nn.ModuleList()
+        for i_level in range(self.num_resolutions):
+            block, attn = nn.ModuleList(), nn.ModuleList()
+            block_in = ch * in_ch_mult[i_level]
+            block_out = ch * ch_mult[i_level]
+            for _ in range(self.num_res_blocks):
+                block.append(ResnetBlock(in_channels=block_in, out_channels=block_out, temb_channels=self.temb_ch, dropout=dropout))
+                block_in = block_out
+                if curr_res in attn_resolutions:
+                    attn.append(AttnBlock(block_in))
+            down = nn.Module()
+            down.block = block
+            down.attn = attn
+            if i_level != self.num_resolutions - 1:
+                down.downsample = Downsample(block_in, resamp_with_conv)
+                curr_res = curr_res // 2
+            self.down.append(down)
+        self.mid = nn.Module()
+        self.mid.block_1 = ResnetBlock(in_channels=block_in, out_channels=block_in, temb_channels=self.temb_ch, dropout=dropout)
+        self.mid.attn_1 = AttnBlock(block_in)
+        self.mid.block_2 = ResnetBlock(in_channels=block_in, out_channels=block_in, temb_channels=self.temb_ch, dropout=dropout)
+        self.norm_out = Normalize(block_in)
+        self.conv_out = nn.Conv2d(block_in, z_channels, kernel_size=3, stride=1, padding=1)
+
+    def forward(self, x):
+        if not tracing():
+            raise RuntimeError("diff_pruning_b200: the Encoder runs on the engine through VQModelInterface.encode (CPU execution exists "
+                               "only under models.trace_mode())")
+        h = self.conv_in(x)
+        for i_level in range(self.num_resolutions):
+            for i_block in range(self.num_res_blocks):
+                h = self.down[i_level].block[i_block](h)
+                if len(self.down[i_level].attn) > 0:
+                    h = self.down[i_level].attn[i_block](h)
+            if i_level != self.num_resolutions - 1:
+                h = self.down[i_level].downsample(h)
+        h = self.mid.block_2(self.mid.attn_1(self.mid.block_1(h)))
+        return self.conv_out(_silu(self.norm_out(h)))
 
 
 class Decoder(nn.Module):
@@ -160,6 +232,30 @@ class Decoder(nn.Module):
         return self.conv_out(_silu(self.norm_out(h)))
 
 
+class _EncodePath(nn.Module):
+    """encoder -> quant_conv of a VQModelInterface (its encode()): the module an encoder plan is built from (engine.Plan._build_vq_encoder).
+    It shares the interface's parameters and is not part of its module tree or state dict."""
+
+    def __init__(self, encoder, quant_conv):
+        super().__init__()
+        self.encoder, self.quant_conv = encoder, quant_conv
+
+
+def _capture(body, device) -> torch.cuda.CUDAGraph:
+    """body() captured as one CUDA graph, after one warm-up run outside the capture (lazy module loading)."""
+    dev = torch.device(device)
+    side = torch.cuda.Stream(device=dev)
+    side.wait_stream(torch.cuda.current_stream(dev))
+    with torch.cuda.stream(side):
+        body()
+    torch.cuda.current_stream(dev).wait_stream(side)
+    torch.cuda.synchronize(dev)
+    g = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(g):
+        body()
+    return g
+
+
 class VectorQuantizer(nn.Module):
     """taming's VectorQuantizer2 as the decode path uses it: the codebook `embedding` ([n_e, e_dim], initialised U(-1/n_e, 1/n_e)).
     The nearest code is chosen by dp_vq_quantize's fp64 distance (include/dpb200.h); remap / sane_index_shape are not supported."""
@@ -174,29 +270,106 @@ class VectorQuantizer(nn.Module):
 
 
 class VQModelInterface(nn.Module):
-    """autoencoder.py:264-282 (VQModel's constructor, :14-43), decode side: `decoder`, `quantize`, `post_quant_conv` in the reference's
-    construction and state-dict order.  decode() runs on the engine in micro-batches of `decode_batch` latents."""
+    """autoencoder.py:264-282 (VQModel's constructor, :14-43): `encoder` (with_encoder=True), `decoder`, `quantize`, `quant_conv`
+    (with_encoder=True) and `post_quant_conv` in the reference's construction and state-dict order, so with the encoder a seeded
+    VQModelInterface draws the reference's parameters (its loss, torch.nn.Identity for cin256-v2, holds none).  decode() and encode() run
+    on the engine in micro-batches of `decode_batch` latents / `encode_batch` images."""
 
     def __init__(self, embed_dim, ddconfig, lossconfig=None, n_embed=8192, ckpt_path=None, ignore_keys=(), image_key="image",
-                 colorize_nlabels=None, monitor=None, remap=None, sane_index_shape=False, use_ema=False, **unused):
+                 colorize_nlabels=None, monitor=None, remap=None, sane_index_shape=False, use_ema=False, with_encoder=False, **unused):
         super().__init__()
         if ckpt_path is not None or colorize_nlabels is not None or use_ema:
             raise NotImplementedError("VQModelInterface ckpt_path / colorize_nlabels / use_ema")
         self.embed_dim, self.n_embed, self.image_key = embed_dim, n_embed, image_key
+        if with_encoder:
+            self.encoder = Encoder(**ddconfig)
         self.decoder = Decoder(**ddconfig)
         self.quantize = VectorQuantizer(n_embed, embed_dim, beta=0.25, remap=remap, sane_index_shape=sane_index_shape)
+        if with_encoder:
+            self.quant_conv = nn.Conv2d(ddconfig["z_channels"], embed_dim, 1)
         self.post_quant_conv = nn.Conv2d(embed_dim, ddconfig["z_channels"], 1)
         self.decode_batch = DECODE_MICRO_BATCH
+        self.encode_batch = ENCODE_MICRO_BATCH
 
     def __getstate__(self):
         d = self.__dict__.copy()
         d.pop("_dpb200_decode", None)
+        d.pop("_dpb200_encode", None)
         return d
 
     use_graph = True     # tests clear it on an instance to run the launch list eagerly
 
+    @torch.no_grad()
     def encode(self, x):
-        raise NotImplementedError("the VQ encoder is not built (only the decode side of the first stage is on the evaluation path)")
+        """autoencoder.py:269-272: quant_conv(encoder(x)), no quantisation.  x: (B, in_channels, H, W) fp32 on CUDA, H and W multiples of
+        2^(len(ch_mult) - 1) (the reference's F.pad + stride-2 convolution takes odd sides too; the engine's does not).  Returns
+        (B, embed_dim, H / 4, W / 4) for VQ-f4."""
+        if not hasattr(self, "encoder"):
+            raise NotImplementedError("this VQModelInterface was built without its encoder: pass with_encoder=True")
+        if tracing():
+            return self.quant_conv(self.encoder(x))
+        if not x.is_cuda:
+            raise RuntimeError("diff_pruning_b200: VQModelInterface.encode runs on a CUDA device (no CPU fallback)")
+        if x.dtype != torch.float32:
+            raise TypeError(f"diff_pruning_b200: the encoder computes in fp32; got {x.dtype}")
+        f = 2 ** (self.encoder.num_resolutions - 1)
+        B, _, H, W = x.shape
+        if H % f or W % f:
+            raise NotImplementedError(f"the engine's encoder takes images whose sides are multiples of {f}; got {H} x {W}")
+        out = None
+        for s in range(0, B, self.encode_batch):
+            run = self.encode_chunk(x[s:s + self.encode_batch])
+            y = run.plan.y_out
+            if out is None:
+                out = torch.empty((B, y.C, y.H, y.W), device=x.device, dtype=torch.float32)
+            n = min(self.encode_batch, B - s)
+            L.check(run.lib.dp_nhwc_to_nchw(y.ptr, y.ld, out[s:s + n].data_ptr(), n, y.C, y.H, y.W, 0, _stream()), "nhwc->nchw")
+        return out
+
+    def encode_chunk(self, x) -> SimpleNamespace:
+        """Encode up to encode_batch images into the micro-batch plan's output buffer (`.plan.y_out`, padded NHWC) and return the runner.
+        A short chunk is padded with zero images, for the reason decode_chunk gives."""
+        n, _, H, W = x.shape
+        assert 0 < n <= self.encode_batch
+        run = self._encode_runner(H, W, x.device)
+        run.x[:n].copy_(x, non_blocking=True)
+        if n < run.x.shape[0]:
+            run.x[n:].zero_()
+        run.plan.ensure_packed()
+        if run.graph is not None:
+            run.graph.replay()
+        else:
+            run.body()
+        return run
+
+    def _encode_runner(self, H, W, device) -> SimpleNamespace:
+        """The encoder plan at (encode_batch, H, W) and its captured graph (dp_nchw_to_nhwc into the plan's input, then the forward); a
+        different request, or parameters replaced since, frees the old plan first."""
+        key = (self.encode_batch, H, W, str(device), self.use_graph)
+        sig = tuple((p.data_ptr(), tuple(p.shape)) for m in (self.encoder, self.quant_conv) for p in m.parameters())
+        run = self.__dict__.get("_dpb200_encode")
+        if run is not None and run.key == key and run.plan.signature() == sig:
+            return run
+        self.__dict__.pop("_dpb200_encode", None)
+        run = None
+        gc.collect()
+        torch.cuda.empty_cache()
+        lib = L.load()
+        B = self.encode_batch
+        plan = Plan(_EncodePath(self.encoder, self.quant_conv), B, H, W, device, need_grad=False)
+        run = SimpleNamespace(key=key, plan=plan, lib=lib, graph=None)
+        run.x = torch.zeros((B, self.encoder.in_channels, H, W), device=device, dtype=torch.float32)
+        x_in = plan.x_in
+
+        def body():
+            L.check(lib.dp_nchw_to_nhwc(run.x.data_ptr(), x_in.ptr, x_in.ld, B, x_in.C, H, W, _stream()), "nchw->nhwc")
+            plan.run_forward()
+        run.body = body
+        plan.ensure_packed()
+        if self.use_graph:
+            run.graph = _capture(body, device)
+        self.__dict__["_dpb200_encode"] = run
+        return run
 
     @torch.no_grad()
     def decode(self, h, force_not_quantize=False, inv_scale: float = 1.0):
@@ -268,17 +441,7 @@ class VQModelInterface(nn.Module):
         run.body = body
         plan.ensure_packed()
         if self.use_graph:
-            dev = torch.device(device)
-            side = torch.cuda.Stream(device=dev)
-            side.wait_stream(torch.cuda.current_stream(dev))
-            with torch.cuda.stream(side):      # warm-up outside capture (lazy module loading)
-                body()
-            torch.cuda.current_stream(dev).wait_stream(side)
-            torch.cuda.synchronize(dev)
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):
-                body()
-            run.graph = g
+            run.graph = _capture(body, device)
         self.__dict__["_dpb200_decode"] = run
         return run
 

@@ -1114,6 +1114,8 @@ class Plan:
             return self._build_ldm()
         if hasattr(self.model, "post_quant_conv"):   # VQ first-stage decoder (autoencoder.py)
             return self._build_vq_decoder()
+        if hasattr(self.model, "quant_conv"):        # VQ first-stage encoder (autoencoder._EncodePath)
+            return self._build_vq_encoder()
         m = self.model
         H, W = self.H, self.W
         cfg = m.config
@@ -1438,12 +1440,25 @@ class Plan:
         self._attn_core(q, k, v, o, float(int(Cc) ** -0.5))
         self.conv(o, m.proj_out.weight, m.proj_out.bias, out, pad=0, residual=x)
 
+    def _vq_resnet(self, rb, x: View) -> View:
+        """ResnetBlock (model.py:82-141) in the attribute vocabulary of Plan.resnet(), into a new buffer."""
+        from types import SimpleNamespace as NS
+        y = self.new(x.N, x.H, x.W, rb.out_channels)
+        self.resnet(NS(norm1=rb.norm1, conv1=rb.conv1, time_emb_proj=None, norm2=rb.norm2, dropout=rb.dropout, conv2=rb.conv2,
+                       conv_shortcut=getattr(rb, "nin_shortcut", None), output_scale_factor=1.0), x, y)
+        return y
+
+    def _vq_attention_new(self, ab, x: View) -> View:
+        """AttnBlock into a new buffer."""
+        y = self.new(x.N, x.H, x.W, x.C)
+        self.vq_attention(ab, x, y)
+        return y
+
     def _build_vq_decoder(self):
         """VQModelInterface.decode after the codebook lookup (autoencoder.py:279-281) and Decoder.forward (model.py:535-568) as a
         forward-only plan: post_quant_conv -> conv_in -> mid (resnet, attention, resnet) -> per level, resnets (+ attention) and nearest x2
         + 3x3 conv -> GroupNorm + SiLU -> conv_out.  B, H, W are the latent's; x_in (the quantised latent, written by dp_vq_quantize) and
         y_out (the decoded images) are padded NHWC buffers."""
-        from types import SimpleNamespace as NS
         if self.need_grad:
             raise NotImplementedError("the VQ decoder plan is forward-only: build it with need_grad=False")
         m = self.model
@@ -1455,18 +1470,7 @@ class Plan:
         self.conv(self.x_in, m.post_quant_conv.weight, m.post_quant_conv.bias, z, pad=0)
         x = self.new(B, H, W, dec.conv_in.out_channels)
         self.conv(z, dec.conv_in.weight, dec.conv_in.bias, x)
-
-        def resnet(rb, x: View) -> View:     # ResnetBlock (model.py:82-141) in the attribute vocabulary of Plan.resnet()
-            y = self.new(x.N, x.H, x.W, rb.out_channels)
-            self.resnet(NS(norm1=rb.norm1, conv1=rb.conv1, time_emb_proj=None, norm2=rb.norm2, dropout=rb.dropout, conv2=rb.conv2,
-                           conv_shortcut=getattr(rb, "nin_shortcut", None), output_scale_factor=1.0), x, y)
-            return y
-
-        def attention(ab, x: View) -> View:
-            y = self.new(x.N, x.H, x.W, x.C)
-            self.vq_attention(ab, x, y)
-            return y
-
+        resnet, attention = self._vq_resnet, self._vq_attention_new
         x = resnet(dec.mid.block_2, attention(dec.mid.attn_1, resnet(dec.mid.block_1, x)))
         for i_level in reversed(range(len(dec.up))):
             lvl = dec.up[i_level]
@@ -1483,6 +1487,43 @@ class Plan:
         self.gn(x, dec.norm_out, a, silu=True)
         self.y_out = self._padded(B, x.H, x.W, dec.conv_out.out_channels)
         self.conv(a, dec.conv_out.weight, dec.conv_out.bias, self.y_out)
+        self._finalize_build()
+
+    def _build_vq_encoder(self):
+        """VQModelInterface.encode (autoencoder.py:269-272) = quant_conv(Encoder.forward) (model.py:428-460) as a forward-only plan:
+        conv_in -> per level, resnets (+ attention) and, below the last level, Downsample -> mid (resnet, attention, resnet) -> GroupNorm
+        + SiLU -> conv_out -> quant_conv.  Downsample's F.pad(x, (0, 1, 0, 1)) + 3x3 stride-2 convolution without padding is the box
+        kernel's stride-2 geometry with pad_t = pad_l = 0: the output grid is the input grid / 2, so the taps that reach the bottom row /
+        right column read past the image and get TMA's zero fill, which is the padding.  B, H, W are the images'; x_in (the images) and
+        y_out (the latents) are padded NHWC buffers."""
+        if self.need_grad:
+            raise NotImplementedError("the VQ encoder plan is forward-only: build it with need_grad=False")
+        m = self.model
+        enc = m.encoder
+        B, H, W = self.B, self.H, self.W
+        self.grad_arena = torch.zeros(0, device=self.dev)
+        self.x_in = self._padded(B, H, W, enc.conv_in.in_channels)
+        x = self.new(B, H, W, enc.conv_in.out_channels)
+        self.conv(self.x_in, enc.conv_in.weight, enc.conv_in.bias, x)
+        resnet, attention = self._vq_resnet, self._vq_attention_new
+        for lvl in enc.down:
+            for i_block, rb in enumerate(lvl.block):
+                x = resnet(rb, x)
+                if len(lvl.attn) > 0:
+                    x = attention(lvl.attn[i_block], x)
+            if hasattr(lvl, "downsample"):
+                d = lvl.downsample.conv
+                assert x.H % 2 == 0 and x.W % 2 == 0, (x.H, x.W)
+                y = self.new(x.N, x.H // 2, x.W // 2, d.out_channels)
+                self.conv(x, d.weight, d.bias, y, stride=2, pad=0)
+                x = y
+        x = resnet(enc.mid.block_2, attention(enc.mid.attn_1, resnet(enc.mid.block_1, x)))
+        a = self.new(x.N, x.H, x.W, x.C)
+        self.gn(x, enc.norm_out, a, silu=True)
+        h = self._padded(B, x.H, x.W, enc.conv_out.out_channels)       # quant_conv's C = 3 operand: pad channels zero
+        self.conv(a, enc.conv_out.weight, enc.conv_out.bias, h)
+        self.y_out = self._padded(B, x.H, x.W, m.quant_conv.out_channels)
+        self.conv(h, m.quant_conv.weight, m.quant_conv.bias, self.y_out, pad=0)
         self._finalize_build()
 
     # ------------------------------------------------------------------ execution

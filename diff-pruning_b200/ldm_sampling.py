@@ -3,13 +3,15 @@
 ClassEmbedder    — ldm/modules/encoders/modules.py:21-33 (`embedding.weight`), the cin256-v2 conditioning (1001 classes, 1000 = unconditional).
 LatentDiffusion  — a thin container of what the loop uses of ldm/models/diffusion/ddpm.py's LatentDiffusion: `model.diffusion_model` (the
                    UNetModel of ldm.py), `cond_stage_model`, the schedule buffers, get_learned_conditioning / apply_model / get_loss_at_t,
-                   and load_state_dict of a Lightning checkpoint's `state_dict`.  Not a Lightning module; no EMA; the
-                   decode side of the VQ first stage (`first_stage_model`, decode_first_stage) when built with first_stage_config.
+                   and load_state_dict of a Lightning checkpoint's `state_dict`.  Not a Lightning module; no EMA; the VQ first
+                   stage (`first_stage_model`: decode_first_stage, and encode_first_stage / get_first_stage_encoding when it holds
+                   its encoder) when built with first_stage_config.
 DDIMSampler      — ldm/models/diffusion/ddim.py: the same `sample(...)` call and results.  The whole S-step sample is ONE CUDA graph: per
                    step a fill of the timestep, the no-grad plan's forward at batch 2B (unconditional | conditional), and dp_ddim_cfg_step,
                    which forms the guided eps, writes x_prev and feeds both halves of the next forward's input.
 LDMPruneScorer   — the loop itself: classes -> guided DDIM-20 sample -> get_loss_at_t at t = iteration on the samples with fresh noise ->
-                   the stop rule of --pruner diff-pruning / diff0 -> backward into the UNet's gradient arena.
+                   the stop rule of --pruner diff-pruning / diff0 -> backward into the UNet's gradient arena.  With encode_samples=True it
+                   is test_criterion.py's loop instead: the samples go through encode_first_stage before get_loss_at_t.
 sample_for_fid   — sample_for_FID.py's render-and-score loop: guided DDIM samples, decode_first_stage on the engine (autoencoder.py), the
                    save_image bytes on the device, FID moments of those bytes and / or the PNG files.
 
@@ -117,8 +119,9 @@ class LatentDiffusion(nn.Module):
     def __init__(self, unet_config: Optional[dict] = None, cond_stage_config: Optional[dict] = None, timesteps: int = 1000,
                  linear_start: float = 0.0015, linear_end: float = 0.0195, cond_stage_key: str = "class_label",
                  first_stage_config: Optional[dict] = None, scale_factor: float = 1.0):
-        """first_stage_config: VQModelInterface's parameters (autoencoder.VQ_F4_CONFIG for cin256-v2) to hold the decode side of the
-        first stage as `first_stage_model`; None (the default) leaves it out, as the latent-space loops need it not."""
+        """first_stage_config: VQModelInterface's parameters (autoencoder.VQ_F4_CONFIG for cin256-v2, plus with_encoder=True for the encode
+        side) to hold the first stage as `first_stage_model`; None (the default) leaves it out, as the latent-space loops need it not.
+        scale_factor: the config's (cin256-v2 leaves it at 1.0)."""
         super().__init__()
         self.model = DiffusionWrapper(UNetModel(**(unet_config or CIN256_V2_CONFIG)))
         self.scale_factor = scale_factor        # ddpm.py:456-457 (scale_by_std False: a plain attribute, not in the state dict)
@@ -142,12 +145,15 @@ class LatentDiffusion(nn.Module):
     def load_state_dict(self, state_dict, strict: bool = True):
         """A Lightning checkpoint's `state_dict` (prune_ldm.py:21-28): `model.diffusion_model.*`, `cond_stage_model.*` and the three
         schedule buffers are loaded; `first_stage_model.*` (the VQ-f4 autoencoder), `model_ema.*` and the schedule buffers this container
-        does not hold are ignored.  With a first stage, its `quantize.*`, `post_quant_conv.*` and `decoder.*` load too (its encoder,
-        quant_conv and loss are not built)."""
+        does not hold are ignored.  With a first stage, its `quantize.*`, `post_quant_conv.*` and `decoder.*` load too, and its
+        `encoder.*` and `quant_conv.*` when it was built with its encoder (its loss is not built)."""
         own = set(self.state_dict().keys())
         prefixes = ("model.diffusion_model.", "cond_stage_model.")
         if hasattr(self, "first_stage_model"):
-            prefixes += tuple(f"first_stage_model.{m}." for m in ("quantize", "post_quant_conv", "decoder"))
+            parts = ("quantize", "post_quant_conv", "decoder")
+            if hasattr(self.first_stage_model, "encoder"):
+                parts += ("encoder", "quant_conv")
+            prefixes += tuple(f"first_stage_model.{m}." for m in parts)
         keep = {k: v for k, v in state_dict.items() if k.startswith(prefixes) or (k in own and "." not in k)}
         return super().load_state_dict(keep, strict=strict)
 
@@ -167,6 +173,22 @@ class LatentDiffusion(nn.Module):
             raise RuntimeError("this LatentDiffusion was built without first_stage_config: it holds no decoder")
         inv = float(torch.tensor(1. / self.scale_factor, dtype=torch.float32))   # the fp32 scalar of `1. / self.scale_factor * z`
         return self.first_stage_model.decode(z, force_not_quantize=predict_cids or force_not_quantize, inv_scale=inv)
+
+    @torch.no_grad()
+    def encode_first_stage(self, x):
+        """ddpm.py:826-863 without the patch-wise path: first_stage_model.encode on the engine (quant_conv(encoder(x)), no quantisation)."""
+        if hasattr(self, "split_input_params"):
+            raise NotImplementedError("patch-wise encoding (split_input_params)")
+        if not hasattr(self, "first_stage_model"):
+            raise RuntimeError("this LatentDiffusion was built without first_stage_config: it holds no encoder")
+        return self.first_stage_model.encode(x)
+
+    def get_first_stage_encoding(self, encoder_posterior):
+        """ddpm.py:542-549 for the VQ first stage, whose encode() returns a tensor: scale_factor * z (the KL first stage's
+        DiagonalGaussianDistribution is not built)."""
+        if not torch.is_tensor(encoder_posterior):
+            raise NotImplementedError(f"encoder_posterior of type '{type(encoder_posterior)}' not yet implemented")
+        return self.scale_factor * encoder_posterior
 
     def get_learned_conditioning(self, c):
         """ddpm.py get_learned_conditioning with the ClassEmbedder: {cond_stage_key: (B,) labels} -> (B, 1, embed_dim)."""
@@ -374,10 +396,17 @@ class LDMPruneScorer:
     """The fast path of prune_ldm.py:105-131: per iteration t = 0, 1, ...: B random classes (`class_sampler(B)`, by default
     random.sample(range(1000), B) on the module-level `random` as the script does), their context, a guided DDIM sample of B latents
     (DDIMSampler: one graph replay), then get_loss_at_t(samples, t, fresh noise) as two graphs — forward + loss, whose loss is read back
-    to the host for the stop rule, and the backward, which accumulates into the UNet's Parameter.grad (the plan's gradient arena)."""
+    to the host for the stop rule, and the backward, which accumulates into the UNet's Parameter.grad (the plan's gradient arena).
+
+    encode_samples=True runs test_criterion.py:108-135 instead: the same loop with encoded = encode_first_stage(samples) (the encoder
+    plan's graph, autoencoder.py) between the sample and get_loss_at_t, which then scores the encoded latents (3 x 16 x 16 for a
+    3 x 64 x 64 cin256-v2 sample) at the same t and with the same stop rule.  The model's first stage must hold its encoder."""
 
     def __init__(self, model: LatentDiffusion, n_samples_per_class: int = 6, ddim_steps: int = 20, scale: float = 3.0, eta: float = 0.0,
-                 use_graph: bool = True):
+                 use_graph: bool = True, encode_samples: bool = False):
+        if encode_samples and not hasattr(getattr(model, "first_stage_model", None), "encoder"):
+            raise ValueError("encode_samples=True needs a first stage built with its encoder (first_stage_config with_encoder=True)")
+        self.encode_samples = encode_samples
         self.model = model
         self.B, self.S, self.scale, self.eta = n_samples_per_class, ddim_steps, float(scale), float(eta)
         self.unet = model.model.diffusion_model
@@ -431,8 +460,9 @@ class LDMPruneScorer:
 
     def run(self, pruner: str = "taylor", iterations: int = 1000, class_sampler: Optional[Callable[[int], Sequence[int]]] = None,
             generator: Optional[torch.Generator] = None) -> torch.Tensor:
-        """The loop of prune_ldm.py:105-131 for `pruner` in {taylor, diff-pruning, diff0}.  Returns the losses of the iterations that
-        ran (with the stopping one last when the rule stopped the loop, its gradient not accumulated; self.stopped_at is its index)."""
+        """The loop of prune_ldm.py:105-131 (test_criterion.py:108-135 with encode_samples) for `pruner` in {taylor, diff-pruning,
+        diff0}.  Returns the losses of the iterations that ran (with the stopping one last when the rule stopped the loop, its gradient
+        not accumulated; self.stopped_at is its index)."""
         rule = PruneLDMStopRule(pruner)
         model, B = self.model, self.B
         key = model.cond_stage_key
@@ -450,6 +480,8 @@ class LDMPruneScorer:
                     samples, _ = self.sampler.sample(S=self.S, conditioning=c, batch_size=B, shape=list(self.shape), verbose=False,
                                                      unconditional_guidance_scale=self.scale, unconditional_conditioning=uc, eta=self.eta,
                                                      generator=generator)
+                    if self.encode_samples:
+                        samples = model.encode_first_stage(samples)
                     noise = torch.randn(samples.shape, generator=generator, device=gdev, dtype=torch.float32).to(self.dev)
                     ts = self._scorer(samples, noise, c)
                     p = ts.plan

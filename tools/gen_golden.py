@@ -17,6 +17,7 @@ Outputs (all small, committed):
     tests/golden/fid_*             FID Inception fixtures (gen_fid): weight-file layout, features of seeded weights, Frechet cases
     tests/golden/ssim_ref.pt       SSIM fixtures (gen_ssim): uint8 image pairs and utils_image.py's per-channel / per-image SSIM
     tests/golden/vq_decoder_tiny.pt  the LDM's VQ first-stage Decoder (small config and VQ-f4 at a 16 x 16 latent) and nearest-code choices
+    tests/golden/vq_encoder_tiny.pt  the LDM's VQ first-stage Encoder and VQModelInterface.encode (small config and VQ-f4 at 64 x 64)
     tests/golden/ldm_ddim_tiny.pt  guided DDIM sampling of the tiny LDM by ldm_exp's DDIMSampler, every step, and one get_loss_at_t pass
 """
 import argparse
@@ -834,13 +835,44 @@ def gen_vq_decoder():
     print("vq_decoder_tiny.pt", os.path.getsize(os.path.join(OUT, "vq_decoder_tiny.pt")))
 
 
+def gen_vq_encoder():
+    """The LDM's VQ first-stage encode side from the UNMODIFIED reference modules (ldm_exp/ldm/modules/diffusionmodules/model.py's
+    Encoder, ldm/models/autoencoder.py's VQModelInterface through ref_shim.install_vq_model) for the small decoder-fixture config (16 x 16
+    images) and the cin256-v2 VQ-f4 ddconfig (64 x 64 images, the size of a cin256-v2 latent sample: 16 x 16 output, 256 attention
+    tokens): the state-dict keys and digests of the seed-s Encoder (torch.manual_seed(s); Encoder(**cfg)) and of the seed-s
+    VQModelInterface (lossconfig torch.nn.Identity, as cin256-v2), two seeded inputs in [-1, 1] and the reference outputs of
+    Encoder.forward and VQModelInterface.encode."""
+    ref_shim.install_vq_model()
+    from ldm.models.autoencoder import VQModelInterface as RefVQ
+    from ldm.modules.diffusionmodules.model import Encoder as RefEncoder
+    from diff_pruning_b200.autoencoder import VQ_F4_CONFIG
+    from oracle import vq_oracle as vo
+    out = {"configs": {}}
+    for name, ddcfg, hw, n_embed, seed in (("tiny", VQ_TINY_DDCONFIG, 16, 64, 0), ("vq_f4", dict(VQ_F4_CONFIG["ddconfig"]), 64, 8192, 1)):
+        torch.manual_seed(seed)
+        enc = RefEncoder(**ddcfg).eval()
+        torch.manual_seed(seed)
+        vq = RefVQ(embed_dim=ddcfg["z_channels"], n_embed=n_embed, ddconfig=ddcfg, lossconfig={"target": "torch.nn.Identity"}).eval()
+        g = torch.Generator().manual_seed(200 + seed)
+        x = torch.rand(2, ddcfg["in_channels"], hw, hw, generator=g) * 2 - 1
+        with torch.no_grad():
+            y, z = enc(x), vq.encode(x)
+        out["configs"][name] = {"ddconfig": ddcfg, "seed": seed, "n_embed": n_embed, "hw": hw,
+                                "sd_keys": list(enc.state_dict().keys()), "digest": vo.state_dict_digest(enc.state_dict()),
+                                "vq_sd_keys": list(vq.state_dict().keys()), "vq_digest": vo.state_dict_digest(vq.state_dict()),
+                                "x": x, "out": y.detach(), "encoded": z.detach()}
+        print("vq_encoder", name, tuple(z.shape), float(y.abs().max()), float(z.abs().max()))
+    torch.save(out, os.path.join(OUT, "vq_encoder_tiny.pt"))
+    print("vq_encoder_tiny.pt", os.path.getsize(os.path.join(OUT, "vq_encoder_tiny.pt")))
+
+
 if __name__ == "__main__":
     ap = argparse.ArgumentParser()
     ap.add_argument("--skip-cfg1", action="store_true")
     ap.add_argument("--only", default=None)
     a = ap.parse_args()
     torch.set_num_threads(os.cpu_count())
-    jobs = {"vq_decoder": gen_vq_decoder, "ssim": gen_ssim, "fid": gen_fid,"ldm_tiny": gen_ldm_tiny, "ldm_ddim": gen_ldm_ddim, "exp_importance": gen_exp_importance, "ref_pickle": gen_ref_pickle, "lsun_struct": gen_lsun_struct, "lr": gen_lr, "ckpt": gen_ckpt, "ddim": gen_ddim, "tiny": gen_tiny, "blocks": gen_blocks, "finetune": gen_finetune, "cifar_fwd": gen_cifar_fwd,
+    jobs = {"vq_encoder": gen_vq_encoder, "vq_decoder": gen_vq_decoder, "ssim": gen_ssim, "fid": gen_fid,"ldm_tiny": gen_ldm_tiny, "ldm_ddim": gen_ldm_ddim, "exp_importance": gen_exp_importance, "ref_pickle": gen_ref_pickle, "lsun_struct": gen_lsun_struct, "lr": gen_lr, "ckpt": gen_ckpt, "ddim": gen_ddim, "tiny": gen_tiny, "blocks": gen_blocks, "finetune": gen_finetune, "cifar_fwd": gen_cifar_fwd,
             "cfg1_s3": gen_cfg1_s3, "cfg3_s3": gen_cfg3_s3, "cfg1": gen_cfg1}
     for name, fn in jobs.items():
         if a.only and name != a.only:

@@ -58,6 +58,29 @@ def install_ldm():
         sys.modules.setdefault(name, types.ModuleType(name))
 
 
+def install_vq_model():
+    """Makes ldm/models/autoencoder.py importable: pytorch_lightning and taming-transformers are not in the build container.
+    LightningModule is stood in by nn.Module, and taming's VectorQuantizer2 by a module that builds what its constructor builds as
+    recalled (taming is not in the reference tree): `embedding` = nn.Embedding(n_e, e_dim) re-drawn U(-1/n_e, 1/n_e), so a seeded
+    VQModelInterface draws its parameters in the reference's order.  encode() does not use the quantizer."""
+    import torch.nn as nn
+    install_ldm()
+    pl = types.ModuleType("pytorch_lightning")
+    pl.LightningModule = nn.Module
+
+    class VectorQuantizer2(nn.Module):
+        def __init__(self, n_e, e_dim, beta, remap=None, unknown_index="random", sane_index_shape=False, legacy=True):
+            super().__init__()
+            self.n_e, self.e_dim, self.beta, self.legacy = n_e, e_dim, beta, legacy
+            self.embedding = nn.Embedding(self.n_e, self.e_dim)
+            self.embedding.weight.data.uniform_(-1.0 / self.n_e, 1.0 / self.n_e)
+    mods = {n: types.ModuleType(n) for n in ("taming", "taming.modules", "taming.modules.vqvae", "taming.modules.vqvae.quantize")}
+    mods["taming.modules.vqvae.quantize"].VectorQuantizer2 = VectorQuantizer2
+    sys.modules.setdefault("pytorch_lightning", pl)
+    for n, m in mods.items():
+        sys.modules.setdefault(n, m)
+
+
 def cpu_ddim_sampler():
     """The reference's DDIMSampler (ldm/models/diffusion/ddim.py) with a register_buffer that leaves tensors on their device: the
     original moves every tensor buffer to CUDA (ddim.py:18-22).  Everything else, the schedule and the sampling loop, is the unmodified
