@@ -22,7 +22,7 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from . import _lib as L
-from .engine import Plan, _stream
+from .engine import Plan, _stream, capture_graphs
 from .models import tracing
 
 VQ_F4_CONFIG = dict(  # ldm_exp/configs/latent-diffusion/cin256-v2.yaml first_stage_config.params
@@ -241,21 +241,6 @@ class _EncodePath(nn.Module):
         self.encoder, self.quant_conv = encoder, quant_conv
 
 
-def _capture(body, device) -> torch.cuda.CUDAGraph:
-    """body() captured as one CUDA graph, after one warm-up run outside the capture (lazy module loading)."""
-    dev = torch.device(device)
-    side = torch.cuda.Stream(device=dev)
-    side.wait_stream(torch.cuda.current_stream(dev))
-    with torch.cuda.stream(side):
-        body()
-    torch.cuda.current_stream(dev).wait_stream(side)
-    torch.cuda.synchronize(dev)
-    g = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(g):
-        body()
-    return g
-
-
 class VectorQuantizer(nn.Module):
     """taming's VectorQuantizer2 as the decode path uses it: the codebook `embedding` ([n_e, e_dim], initialised U(-1/n_e, 1/n_e)).
     The nearest code is chosen by dp_vq_quantize's fp64 distance (include/dpb200.h); remap / sane_index_shape are not supported."""
@@ -313,63 +298,24 @@ class VQModelInterface(nn.Module):
         if x.dtype != torch.float32:
             raise TypeError(f"diff_pruning_b200: the encoder computes in fp32; got {x.dtype}")
         f = 2 ** (self.encoder.num_resolutions - 1)
-        B, _, H, W = x.shape
+        H, W = x.shape[2:]
         if H % f or W % f:
             raise NotImplementedError(f"the engine's encoder takes images whose sides are multiples of {f}; got {H} x {W}")
-        out = None
-        for s in range(0, B, self.encode_batch):
-            run = self.encode_chunk(x[s:s + self.encode_batch])
-            y = run.plan.y_out
-            if out is None:
-                out = torch.empty((B, y.C, y.H, y.W), device=x.device, dtype=torch.float32)
-            n = min(self.encode_batch, B - s)
-            L.check(run.lib.dp_nhwc_to_nchw(y.ptr, y.ld, out[s:s + n].data_ptr(), n, y.C, y.H, y.W, 0, _stream()), "nhwc->nchw")
-        return out
+        return self._micro_batched(x, self.encode_batch, self.encode_chunk)
 
     def encode_chunk(self, x) -> SimpleNamespace:
         """Encode up to encode_batch images into the micro-batch plan's output buffer (`.plan.y_out`, padded NHWC) and return the runner.
         A short chunk is padded with zero images, for the reason decode_chunk gives."""
         n, _, H, W = x.shape
         assert 0 < n <= self.encode_batch
-        run = self._encode_runner(H, W, x.device)
-        run.x[:n].copy_(x, non_blocking=True)
-        if n < run.x.shape[0]:
-            run.x[n:].zero_()
-        run.plan.ensure_packed()
-        if run.graph is not None:
-            run.graph.replay()
-        else:
-            run.body()
-        return run
-
-    def _encode_runner(self, H, W, device) -> SimpleNamespace:
-        """The encoder plan at (encode_batch, H, W) and its captured graph (dp_nchw_to_nhwc into the plan's input, then the forward); a
-        different request, or parameters replaced since, frees the old plan first."""
-        key = (self.encode_batch, H, W, str(device), self.use_graph)
-        sig = tuple((p.data_ptr(), tuple(p.shape)) for m in (self.encoder, self.quant_conv) for p in m.parameters())
-        run = self.__dict__.get("_dpb200_encode")
-        if run is not None and run.key == key and run.plan.signature() == sig:
-            return run
-        self.__dict__.pop("_dpb200_encode", None)
-        run = None
-        gc.collect()
-        torch.cuda.empty_cache()
-        lib = L.load()
         B = self.encode_batch
-        plan = Plan(_EncodePath(self.encoder, self.quant_conv), B, H, W, device, need_grad=False)
-        run = SimpleNamespace(key=key, plan=plan, lib=lib, graph=None)
-        run.x = torch.zeros((B, self.encoder.in_channels, H, W), device=device, dtype=torch.float32)
-        x_in = plan.x_in
 
-        def body():
-            L.check(lib.dp_nchw_to_nhwc(run.x.data_ptr(), x_in.ptr, x_in.ld, B, x_in.C, H, W, _stream()), "nchw->nhwc")
-            plan.run_forward()
-        run.body = body
-        plan.ensure_packed()
-        if self.use_graph:
-            run.graph = _capture(body, device)
-        self.__dict__["_dpb200_encode"] = run
-        return run
+        def setup(run):        # dp_nchw_to_nhwc of `.x` into the plan's input
+            run.x = torch.zeros((B, self.encoder.in_channels, H, W), device=x.device, dtype=torch.float32)
+            x_in = run.plan.x_in
+            return lambda: L.check(run.lib.dp_nchw_to_nhwc(run.x.data_ptr(), x_in.ptr, x_in.ld, B, x_in.C, H, W, _stream()), "nchw->nhwc")
+        run = self._runner("_dpb200_encode", _EncodePath(self.encoder, self.quant_conv), B, H, W, (), x.device, setup)
+        return self._run_chunk(run, run.x, x)
 
     @torch.no_grad()
     def decode(self, h, force_not_quantize=False, inv_scale: float = 1.0):
@@ -381,17 +327,7 @@ class VQModelInterface(nn.Module):
             raise RuntimeError("diff_pruning_b200: VQModelInterface.decode runs on a CUDA device (no CPU fallback)")
         if h.dtype != torch.float32:
             raise TypeError(f"diff_pruning_b200: the decoder computes in fp32; got {h.dtype}")
-        B, _, H, W = h.shape
-        out = None
-        for s in range(0, B, self.decode_batch):
-            run = self.decode_chunk(h[s:s + self.decode_batch], force_not_quantize, inv_scale)
-            if out is None:
-                y = run.plan.y_out
-                out = torch.empty((B, y.C, y.H, y.W), device=h.device, dtype=torch.float32)
-            n = min(self.decode_batch, B - s)
-            y = run.plan.y_out
-            L.check(run.lib.dp_nhwc_to_nchw(y.ptr, y.ld, out[s:s + n].data_ptr(), n, y.C, y.H, y.W, 0, _stream()), "nhwc->nchw")
-        return out
+        return self._micro_batched(h, self.decode_batch, lambda z: self.decode_chunk(z, force_not_quantize, inv_scale))
 
     def decode_chunk(self, h, force_not_quantize=False, inv_scale: float = 1.0, indices: bool = False) -> SimpleNamespace:
         """Decode up to decode_batch latents into the micro-batch plan's output buffer (`.plan.y_out`, padded NHWC) and return the
@@ -400,50 +336,78 @@ class VQModelInterface(nn.Module):
         codes in `.indices` ([decode_batch, H, W] int64)."""
         n, _, H, W = h.shape
         assert 0 < n <= self.decode_batch
-        run = self._runner(H, W, bool(force_not_quantize), float(inv_scale), h.device)
-        run.z[:n].copy_(h, non_blocking=True)
-        if n < run.z.shape[0]:
-            run.z[n:].zero_()
-        run.plan.ensure_packed()
+        B, fnq, inv_scale = self.decode_batch, bool(force_not_quantize), float(inv_scale)
+
+        def setup(run):        # dp_vq_quantize of `.z` into the plan's input, writing `.indices` when asked to
+            run.z = torch.zeros((B, self.embed_dim, H, W), device=h.device, dtype=torch.float32)
+            run.indices = torch.zeros((B, H, W), device=h.device, dtype=torch.int64)
+            run.want_indices = [False]
+            emb, x_in = self.quantize.embedding.weight, run.plan.x_in
+
+            def stage():
+                idx = run.indices.data_ptr() if (run.want_indices[0] and not fnq) else None
+                L.check(run.lib.dp_vq_quantize(run.z.data_ptr(), B, self.embed_dim, H, W, inv_scale, emb.data_ptr(), self.n_embed,
+                                               0 if fnq else 1, x_in.ptr, x_in.ld, idx, _stream()), "vq_quantize")
+            return stage
+        run = self._runner("_dpb200_decode", self, B, H, W, (fnq, inv_scale), h.device, setup)
         run.want_indices[0] = indices
-        if run.graph is not None and not indices:
+        return self._run_chunk(run, run.z, h, eager=indices)
+
+    def _runner(self, slot, module, B, H, W, extra, device, setup) -> SimpleNamespace:
+        """The forward-only plan of `module` at (B, H, W), kept in __dict__[slot], and with use_graph its captured graph.  setup(run)
+        allocates the runner's input buffers and returns the staging launch into the plan's input; run.body() is that launch, then the
+        forward.  A different request (`extra` holds what else the staging launch depends on), or parameters replaced since, frees the
+        old plan first."""
+        key = (B, H, W, *extra, str(device), self.use_graph)
+        sig = tuple((p.data_ptr(), tuple(p.shape)) for p in module.parameters())
+        run = self.__dict__.get(slot)
+        if run is not None and run.key == key and run.plan.signature() == sig:
+            return run
+        self.__dict__.pop(slot, None)
+        run = None
+        gc.collect()
+        torch.cuda.empty_cache()
+        plan = Plan(module, B, H, W, device, need_grad=False)
+        run = SimpleNamespace(key=key, plan=plan, lib=L.load(), graph=None)
+        stage = setup(run)
+
+        def body():
+            stage()
+            plan.run_forward()
+        run.body = body
+        plan.ensure_packed()
+        if self.use_graph:
+            run.graph, = capture_graphs(device, body)
+        self.__dict__[slot] = run
+        return run
+
+    @staticmethod
+    def _run_chunk(run, buf, x, eager=False) -> SimpleNamespace:
+        """x into the runner's input buffer, its tail zeroed for a short chunk, then one graph replay (or body() when eager)."""
+        n = x.shape[0]
+        buf[:n].copy_(x, non_blocking=True)
+        if n < buf.shape[0]:
+            buf[n:].zero_()
+        run.plan.ensure_packed()
+        if run.graph is not None and not eager:
             run.graph.replay()
         else:
             run.body()
         return run
 
-    def _runner(self, H, W, fnq, inv_scale, device) -> SimpleNamespace:
-        """The decoder plan at (decode_batch, H, W) and its captured graph (dp_vq_quantize into the plan's input, then the forward) for
-        one (force_not_quantize, inv_scale); a different request, or parameters replaced since, frees the old plan first."""
-        key = (self.decode_batch, H, W, fnq, inv_scale, str(device), self.use_graph)
-        sig = tuple((p.data_ptr(), tuple(p.shape)) for p in self.parameters())
-        run = self.__dict__.get("_dpb200_decode")
-        if run is not None and run.key == key and run.plan.signature() == sig:
-            return run
-        self.__dict__.pop("_dpb200_decode", None)
-        run = None
-        gc.collect()
-        torch.cuda.empty_cache()
-        lib = L.load()
-        B = self.decode_batch
-        plan = Plan(self, B, H, W, device, need_grad=False)
-        run = SimpleNamespace(key=key, plan=plan, lib=lib, graph=None, want_indices=[False])
-        run.z = torch.zeros((B, self.embed_dim, H, W), device=device, dtype=torch.float32)
-        run.indices = torch.zeros((B, H, W), device=device, dtype=torch.int64)
-        emb = self.quantize.embedding.weight
-        x_in = plan.x_in
-
-        def body():
-            idx = run.indices.data_ptr() if (run.want_indices[0] and not fnq) else None
-            L.check(lib.dp_vq_quantize(run.z.data_ptr(), B, self.embed_dim, H, W, inv_scale, emb.data_ptr(), self.n_embed,
-                                       0 if fnq else 1, x_in.ptr, x_in.ld, idx, _stream()), "vq_quantize")
-            plan.run_forward()
-        run.body = body
-        plan.ensure_packed()
-        if self.use_graph:
-            run.graph = _capture(body, device)
-        self.__dict__["_dpb200_decode"] = run
-        return run
+    @staticmethod
+    def _micro_batched(x, mb, chunk):
+        """chunk() over micro-batches of mb along x's batch, each chunk's padded NHWC output gathered into one NCHW tensor."""
+        B = x.shape[0]
+        out = None
+        for s in range(0, B, mb):
+            run = chunk(x[s:s + mb])
+            y = run.plan.y_out
+            if out is None:
+                out = torch.empty((B, y.C, y.H, y.W), device=x.device, dtype=torch.float32)
+            n = min(mb, B - s)
+            L.check(run.lib.dp_nhwc_to_nchw(y.ptr, y.ld, out[s:s + n].data_ptr(), n, y.C, y.H, y.W, 0, _stream()), "nhwc->nchw")
+        return out
 
     def _decode_traced(self, h, force_not_quantize, inv_scale):
         """Host restatement used under models.trace_mode(): the same codebook choice as dp_vq_quantize (fp64 distances, lowest index on

@@ -1725,6 +1725,33 @@ class frozen_weights:
         return False
 
 
+def capture_graphs(device, *bodies: Callable[[], None], restore=()) -> List[torch.cuda.CUDAGraph]:
+    """One CUDA graph per body, in the order given.  Every body runs exactly once outside the capture, in order, on a side stream as torch
+    requires (first launches load their modules there, not inside the capture), and is then captured once.  Anything a body accumulates
+    into or updates whose warm-up value must not survive goes in `restore` (None entries are skipped): it is cloned before the warm-up
+    and copied back after it."""
+    dev = torch.device(device)
+    torch.cuda.synchronize(dev)
+    side = torch.cuda.Stream(device=dev)
+    side.wait_stream(torch.cuda.current_stream(dev))
+    with torch.cuda.stream(side):
+        saved = [(t, t.clone()) for t in restore if t is not None]
+        for body in bodies:
+            body()
+        for t, s in saved:
+            t.copy_(s)
+        del saved          # freed before the capture, whose entry empties the allocator's cache
+    torch.cuda.current_stream(dev).wait_stream(side)
+    torch.cuda.synchronize(dev)
+    graphs = []
+    for body in bodies:
+        g = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(g):
+            body()
+        graphs.append(g)
+    return graphs
+
+
 def add_noise_cuda(sched, x0: torch.Tensor, noise: torch.Tensor, timesteps: torch.Tensor) -> torch.Tensor:
     """DDPMScheduler.add_noise on CUDA — scheduling_ddpm.py:408-429."""
     lib = L.load()

@@ -25,7 +25,7 @@ import torch
 import torch.nn as nn
 
 from . import _lib as L
-from .engine import View, _stream
+from .engine import View, _stream, capture_graphs
 
 WEIGHTS_FILE = "pt_inception-2015-12-05-6726825d.pth"
 WEIGHTS_ENV = "DPB200_FID_WEIGHTS"
@@ -432,16 +432,7 @@ class FeaturePlan:
             self.run_eager()
             return
         if self._graph is None:
-            side = torch.cuda.Stream(device=self.dev)
-            side.wait_stream(torch.cuda.current_stream(self.dev))
-            with torch.cuda.stream(side):      # warm-up outside capture (lazy module loading)
-                self.run_eager()
-            torch.cuda.current_stream(self.dev).wait_stream(side)
-            torch.cuda.synchronize(self.dev)
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):
-                self.run_eager()
-            self._graph = g
+            self._graph, = capture_graphs(self.dev, self.run_eager)
         self._graph.replay()
 
 

@@ -32,7 +32,7 @@ import torch.nn as nn
 
 from . import _lib as L
 from .autoencoder import VQModelInterface
-from .engine import _stream, frozen_weights, get_plan
+from .engine import _stream, capture_graphs, frozen_weights, get_plan
 from .ldm import CIN256_V2_CONFIG, UNetModel
 from .scoring import TaylorScorer
 
@@ -345,17 +345,7 @@ class DDIMSampler:
             run.x_T.zero_()
             if run.noise is not None:
                 run.noise.zero_()
-            torch.cuda.synchronize(dev)
-            side = torch.cuda.Stream(device=dev)
-            side.wait_stream(torch.cuda.current_stream(dev))
-            with torch.cuda.stream(side):      # warm-up outside capture (lazy module loading)
-                body()
-            torch.cuda.current_stream(dev).wait_stream(side)
-            torch.cuda.synchronize(dev)
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):
-                body()
-            run.graph = g
+            run.graph, = capture_graphs(dev, body)
         self._graphs[key] = run
         return run
 
@@ -440,24 +430,6 @@ class LDMPruneScorer:
     def _bwd(self):
         self.ts.plan.run_backward(_stream())
 
-    def _capture(self):
-        ts, dev = self.ts, self.dev
-        torch.cuda.synchronize(dev)
-        side = torch.cuda.Stream(device=dev)
-        side.wait_stream(torch.cuda.current_stream(dev))
-        with torch.cuda.stream(side):       # warm-up outside capture (lazy module loading); the gradient arena is restored after it
-            saved = ts.plan.grad_arena.clone()
-            self._fwd()
-            self._bwd()
-            ts.plan.grad_arena.copy_(saved)
-        torch.cuda.current_stream(dev).wait_stream(side)
-        torch.cuda.synchronize(dev)
-        self.g_fwd, self.g_bwd = torch.cuda.CUDAGraph(), torch.cuda.CUDAGraph()
-        with torch.cuda.graph(self.g_fwd):
-            self._fwd()
-        with torch.cuda.graph(self.g_bwd):
-            self._bwd()
-
     def run(self, pruner: str = "taylor", iterations: int = 1000, class_sampler: Optional[Callable[[int], Sequence[int]]] = None,
             generator: Optional[torch.Generator] = None) -> torch.Tensor:
         """The loop of prune_ldm.py:105-131 (test_criterion.py:108-135 with encode_samples) for `pruner` in {taylor, diff-pruning,
@@ -491,7 +463,7 @@ class LDMPruneScorer:
                     p.t_dev.fill_(t)
                     if self.use_graph:
                         if self.g_fwd is None:
-                            self._capture()
+                            self.g_fwd, self.g_bwd = capture_graphs(self.dev, self._fwd, self._bwd, restore=(p.grad_arena,))
                         self.g_fwd.replay()
                     else:
                         self._fwd()

@@ -147,7 +147,7 @@ class DDIMPipeline:
         timesteps = self.scheduler.timesteps.tolist()
         if not image.is_cuda:
             raise RuntimeError("diff_pruning_b200: DDIMPipeline samples on a CUDA device (no CPU fallback); call pipeline.to('cuda')")
-        from .engine import frozen_weights, get_plan
+        from .engine import capture_graphs, frozen_weights, get_plan
         was_training = self.unet.training
         self.unet.eval()
         try:
@@ -163,16 +163,7 @@ class DDIMPipeline:
                         plan.run_forward()
                         L.check(L.load().dp_nhwc_to_nchw(plan.y_out.ptr, plan.y_out.ld, eps.data_ptr(), plan.B, plan.y_out.C, plan.H, plan.W, 0,
                                                          _stream()), "nhwc->nchw")
-                    torch.cuda.synchronize(image.device)
-                    side = torch.cuda.Stream(device=image.device)
-                    side.wait_stream(torch.cuda.current_stream(image.device))
-                    with torch.cuda.stream(side):     # warm-up outside capture (lazy module loading)
-                        body()
-                    torch.cuda.current_stream(image.device).wait_stream(side)
-                    torch.cuda.synchronize(image.device)
-                    graph = torch.cuda.CUDAGraph()
-                    with torch.cuda.graph(graph):
-                        body()
+                    graph, = capture_graphs(image.device, body)
                     for t in timesteps:
                         plan.t_dev.fill_(t)
                         graph.replay()

@@ -21,7 +21,7 @@ import torch
 import torch.nn as nn
 
 from . import _lib as L
-from .engine import Plan, _dropout_seed, _stream, arena_offsets, get_plan, invalidate_packs
+from .engine import Plan, _dropout_seed, _stream, arena_offsets, capture_graphs, get_plan, invalidate_packs
 from .models import UNet2DModel, ddpm_alphas_cumprod
 
 
@@ -89,24 +89,6 @@ class TaylorScorer:
         self._forward_loss()
         self.plan.run_backward(_stream())
 
-    def _capture(self):
-        torch.cuda.synchronize(self.dev)
-        side = torch.cuda.Stream(device=self.dev)
-        side.wait_stream(torch.cuda.current_stream(self.dev))
-        with torch.cuda.stream(side):   # warm-up outside capture (first-launch lazy module loading)
-            saved = self.plan.grad_arena.clone()
-            saved_sc = self.plan.score_arena.clone() if self.plan.fused_scores else None
-            self._body()
-            self.plan.grad_arena.copy_(saved)
-            if saved_sc is not None:
-                self.plan.score_arena.copy_(saved_sc)
-        torch.cuda.current_stream(self.dev).wait_stream(side)
-        torch.cuda.synchronize(self.dev)
-        g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g):
-            self._body()
-        self.graph = g
-
     def signed_scores(self) -> Dict[str, Tuple[torch.Tensor, torch.Tensor]]:
         """{weight name: (out-channel, in-channel) sum_t sum_k W*dW_t} accumulated by the fused reduce (fused_scores=True)."""
         names = {id(p): n for n, p in self.model.named_parameters()}
@@ -124,9 +106,8 @@ class TaylorScorer:
             p.t_dev.fill_(int(t))
         if self.use_graph:
             if self.graph is None:
-                tsave = p.t_dev.clone()
-                self._capture()
-                p.t_dev.copy_(tsave)
+                self.graph, = capture_graphs(self.dev, self._body,
+                                             restore=(p.grad_arena, p.score_arena if p.fused_scores else None, p.t_dev))
             self.graph.replay()
         else:
             self._body()
@@ -395,15 +376,6 @@ class FinetuneStepper:
         self._adam_args = a
         L.check(lib.dp_adam_clip_ema(a, s), "adam")
 
-    def _capture(self):
-        torch.cuda.synchronize(self.dev)
-        self.g_main = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(self.g_main):
-            self._main()
-        self.g_tail = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(self.g_tail):
-            self._tail()
-
     def step(self, clean: torch.Tensor, noise: torch.Tensor, timesteps: torch.Tensor) -> torch.Tensor:
         """One optimisation step; returns the device loss scalar (this rank's minibatch)."""
         B, C_, H, W = clean.shape
@@ -420,13 +392,8 @@ class FinetuneStepper:
         self.step_scalars.copy_(bc, non_blocking=True)
         p.dropout_seed_dev.fill_(_dropout_seed(t))   # per step AND per rank: data-parallel ranks draw different masks
         if self.use_graph and self.g_main is None:
-            # warm-up once outside capture (lazy module loading), on a side stream as torch requires
-            side = torch.cuda.Stream(device=self.dev)
-            side.wait_stream(torch.cuda.current_stream(self.dev))
-            with torch.cuda.stream(side):
-                self._main()
-            torch.cuda.current_stream(self.dev).wait_stream(side)
-            self._capture()
+            self.g_main, self.g_tail = capture_graphs(self.dev, self._main, self._tail,
+                                                      restore=(self.param_arena, self.m, self.v, self.ema))
         if self.use_graph:
             self.g_main.replay()
         else:
