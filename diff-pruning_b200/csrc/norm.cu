@@ -754,6 +754,14 @@ __global__ void ln_bwd_param_final_kernel(const dp_gn_args a, const float* __res
 static inline bool ln_fast(const dp_gn_args* a) {     // the row kernels take what the LDM transformer blocks ask for
   return a->HW == 1 && a->G == 1 && a->C % 4 == 0 && a->C <= 4 * 32 * LN_V && !a->silu && a->dropout_p == 0.f && !a->y_bf16;
 }
+// Whether the forward (bwd = false) or backward launch runs on the row kernels: ln_fast plus the float4 access of every view they
+// touch.  Validation admits C > NT * MAXCPT only when this holds: a LayerNorm that misses the row kernels falls onto the GroupNorm
+// kernels, whose channel maps end at NT * MAXCPT channels (make_map4 has no pixel lane left above that).
+static inline bool ln_rows(const dp_gn_args* a, bool bwd) {
+  if (!ln_fast(a) || !al16(a->x, a->ldx) || !al16(a->gamma, 0)) return false;
+  if (bwd) return al16(a->dy, a->lddy) && al16(a->dx, a->lddx) && al16(a->dx_add, a->ldadd) && al16(a->dx_add2, a->ldadd2);
+  return a->y && al16(a->y, a->ldy) && al16(a->beta, 0);
+}
 
 
 static size_t align256(size_t v) { return (v + 255) & ~(size_t)255; }
@@ -770,24 +778,24 @@ extern "C" size_t dp_groupnorm_workspace_bytes(int32_t N, int32_t HW, int32_t C,
   return align256(fwd > bwd ? fwd : bwd);
 }
 
-static int gn_validate(const dp_gn_args* a) {
+static int gn_validate(const dp_gn_args* a, bool bwd) {
   DP_REQUIRE(a && a->x && a->gamma && a->beta && a->mean && a->rstd && a->workspace, DP_ERR_NULL);
   DP_REQUIRE(a->N > 0 && a->HW > 0 && a->C > 0 && a->G > 0 && a->C % a->G == 0, DP_ERR_SHAPE);
-  DP_REQUIRE((a->C <= NT * MAXCPT || ln_fast(a)) && a->G <= 1024, DP_ERR_UNSUPPORTED);
+  DP_REQUIRE((a->C <= NT * MAXCPT || ln_rows(a, bwd)) && a->G <= 1024, DP_ERR_UNSUPPORTED);
   DP_REQUIRE(a->ldx >= a->C, DP_ERR_SHAPE);
   DP_REQUIRE(a->dropout_p >= 0.f && a->dropout_p < 1.f, DP_ERR_SHAPE);
   return DP_OK;
 }
 
 extern "C" int dp_groupnorm_fwd(const dp_gn_args* a, dp_stream_t stream) {
-  int rc = gn_validate(a);
+  DP_REQUIRE(a && (a->y || a->y_bf16), DP_ERR_NULL);     // before validation: a missing output is DP_ERR_NULL at any width
+  int rc = gn_validate(a, false);
   if (rc) return rc;
-  DP_REQUIRE(a->y || a->y_bf16, DP_ERR_NULL);
   DP_REQUIRE(!a->y || a->ldy >= a->C, DP_ERR_SHAPE);
   DP_REQUIRE(!a->y_bf16 || (a->ldyb >= a->C && a->ldyb % 8 == 0 && (((uintptr_t)a->y_bf16) & 15) == 0), DP_ERR_ALIGN);
   cudaStream_t st = (cudaStream_t)stream;
   const bool v4 = (a->C % 4 == 0) && al16(a->x, a->ldx) && al16(a->y, a->ldy);
-  if (v4 && a->y && ln_fast(a) && al16(a->gamma, 0) && al16(a->beta, 0)) {     // LayerNorm over tokens: one warp per row
+  if (ln_rows(a, false)) {     // LayerNorm over tokens: one warp per row
     ln_fwd_kernel<<<(unsigned)((a->N + 7) / 8), 256, 0, st>>>(*a);
     return dp_check_launch();
   }
@@ -816,7 +824,7 @@ extern "C" int dp_groupnorm_fwd(const dp_gn_args* a, dp_stream_t stream) {
 }
 
 extern "C" int dp_groupnorm_bwd(const dp_gn_args* a, dp_stream_t stream) {
-  int rc = gn_validate(a);
+  int rc = gn_validate(a, true);
   if (rc) return rc;
   DP_REQUIRE(a->dy && a->dx, DP_ERR_NULL);
   DP_REQUIRE(a->lddy >= a->C && a->lddx >= a->C, DP_ERR_SHAPE);
@@ -824,7 +832,7 @@ extern "C" int dp_groupnorm_bwd(const dp_gn_args* a, dp_stream_t stream) {
   const bool v4 = (a->C % 4 == 0) && al16(a->x, a->ldx) && al16(a->dy, a->lddy) && al16(a->dx, a->lddx) &&
                   al16(a->dx_add, a->ldadd) && al16(a->dx_add2, a->ldadd2);
   DP_REQUIRE(!(a->fin && ln_fast(a)), DP_ERR_UNSUPPORTED);     // the row kernels take dgamma / dbeta from x and dy, not from fin
-  if (v4 && ln_fast(a) && al16(a->gamma, 0)) {      // LayerNorm over tokens: row kernel for dx, chunked column sums for dgamma / dbeta
+  if (ln_rows(a, true)) {      // LayerNorm over tokens: row kernel for dx, chunked column sums for dgamma / dbeta
     DP_REQUIRE((a->N + LN_ROWS - 1) / LN_ROWS <= 65535, DP_ERR_SHAPE);     // one grid row per chunk of the column sums
     ln_bwd_dx_kernel<<<(unsigned)((a->N + 7) / 8), 256, 0, st>>>(*a);
     if ((rc = dp_check_launch())) return rc;

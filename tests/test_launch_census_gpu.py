@@ -66,10 +66,12 @@ class Buf:
     """A [rows][ld] fp32 (or bf16) buffer whose view of `cols` channels starts at the same 16-byte phase as the captured pointer;
     everything around the view holds `fill`."""
 
+    TAIL_ROWS = 128       # rows of `fill` past the view: a box of pixels running past the batch must not store there
+
     def __init__(self, ptr, rows, ld, cols, fill=SENT, dtype=torch.float32):
         esz = 4 if dtype == torch.float32 else 2
         self.phase = (int(ptr) % 16) // esz
-        self.t = torch.full((rows * ld + 16 // esz,), fill, device="cuda", dtype=dtype)
+        self.t = torch.full(((rows + self.TAIL_ROWS) * ld + 16 // esz,), fill, device="cuda", dtype=dtype)
         self.v = self.t[self.phase:self.phase + rows * ld].view(rows, ld)[:, :cols]
         self.fill = fill
 
@@ -205,7 +207,8 @@ DP_CONV_RELU = 4
 def replay_conv(lib, g, name, a, rep, chain=None):
     """fprop / dgrad (fp32-grade) at the captured geometry.  With DP_CONV_RELU the fp64 reference takes the ReLU after every epilogue
     term (1-Lipschitz: same bound).  chain(args, split-K workspace floats) -> (L, tensor-core launch?) overrides the box kernel's
-    chain length (the general-geometry and SIMT kernels of the evaluation census)."""
+    chain length (the general-geometry and SIMT kernels of the evaluation census).  Returns the split-K workspace the launch was
+    given, NaN-filled before the first run (None without one)."""
     N, H, W, Cin, P, Q, K, R, Sx = a.N, a.H, a.W, a.C, a.P, a.Q, a.K, a.R, a.S
     tc = bool(a.w_tc_hi)
     w, ck, kc, packs = _conv_weights(lib, g, K, Cin, R, Sx, tc)
@@ -280,6 +283,7 @@ def replay_conv(lib, g, name, a, rep, chain=None):
     _check(rep, name, got, ref, lc.product_bound(s, L_, epi), f"{N}x{H}x{W} {Cin}->{K} {R}x{Sx} s{a.stride} L={L_}")
     if so is not None:
         assert _slot_value(so) == float(got.abs().max()), name
+    return ws
 
 
 def replay_wgrad(lib, g, name, a, rep):
