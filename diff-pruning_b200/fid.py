@@ -441,12 +441,13 @@ class Moments:
     """n, sum d and the upper triangle of sum d d^T of a feature stream, d = x - shift, in fp64 on the device.  The shift is the fp32
     mean of the first batch added (dp_global_mean over its rows), so the covariance does not cancel against mu mu^T when features sit far
     from zero.  Moments about one shift add: batches, padded final batches (only the valid rows enter) and, later, devices sharing the
-    shift combine by plain sums."""
+    shift combine by plain sums (share_shift, then all_reduce)."""
 
     def __init__(self, dims: int, device=None):
         dev = device if device is not None else torch.device("cuda", torch.cuda.current_device())
         self.D, self.n = dims, 0
         self.shift = torch.zeros(dims, dtype=torch.float32, device=dev)
+        self.shift_set = False
         self.s = torch.zeros(dims, dtype=torch.float64, device=dev)
         self.sxx = torch.zeros(dims, dims, dtype=torch.float64, device=dev)
 
@@ -454,12 +455,31 @@ class Moments:
         rows = feat.shape[0] if rows is None else rows
         assert feat.dtype == torch.float32 and feat.is_cuda and feat.stride(1) == 1 and feat.shape[1] == self.D
         lib = L.load()
-        if self.n == 0 and rows > 0:      # [rows][D] as one image of rows x 1 pixels
+        if not self.shift_set and rows > 0:      # [rows][D] as one image of rows x 1 pixels
             L.check(lib.dp_global_mean(feat.data_ptr(), feat.stride(0), self.shift.data_ptr(), self.D, 1, rows, 1, self.D, _stream()),
                     "moments shift")
+            self.shift_set = True
         L.check(lib.dp_feature_moments(feat.data_ptr(), feat.stride(0), rows, self.D, self.shift.data_ptr(), self.s.data_ptr(),
                                        self.sxx.data_ptr(), _stream()), "feature_moments")
         self.n += rows
+
+    def share_shift(self, src: int = 0):
+        """Every rank of the default process group takes rank `src`'s shift (one broadcast).  Called by all ranks, after rank src added
+        its first rows and before any other rank added any."""
+        import torch.distributed as dist
+        if dist.get_rank() != src and self.n:
+            raise RuntimeError("share_shift: this rank already added rows about a shift of its own")
+        dist.broadcast(self.shift, src)
+        self.shift_set = True
+
+    def all_reduce(self):
+        """Sums n, s and sxx over the ranks of the default process group, which must share the shift (share_shift): every rank then
+        holds the moments of all their rows."""
+        import torch.distributed as dist
+        n = torch.tensor([self.n], dtype=torch.int64, device=self.s.device)
+        for t in (n, self.s, self.sxx):
+            dist.all_reduce(t, op=dist.ReduceOp.SUM)
+        self.n = int(n.item())
 
     def finalize(self):
         """(mu, sigma) as np.mean(act, 0) and np.cov(act, rowvar=False) define them, float64."""

@@ -17,6 +17,14 @@ sample_for_fid   — sample_for_FID.py's render-and-score loop: guided DDIM samp
 
 Gradients reach the UNet only: the reference's trainable ClassEmbedder also gets a gradient from loss.backward(), but the pruner looks at
 `diffusion_model` alone, and the context enters the engine as a constant input.
+
+Under torch.distributed with W > 1 ranks (one process per GPU, torchrun) both loops shard and return the single-process result on every
+rank.  They run in rounds of W consecutive iterations (LDMPruneScorer) or batches (sample_for_fid), rank r taking the r-th of each round.
+Rank 0 draws the round's random inputs (class labels, x_T, per-step noise, q_sample noise) in the single-process order and broadcasts
+each iteration's draws, so no other rank's random state is read.  LDMPruneScorer all-reduces the round's losses and every rank replays
+the stop rule over them in iteration order; the gradient arena is all-reduced once at the end.  sample_for_fid shares the FID moments'
+shift (rank 0's first batch) and all-reduces the moments once at the end.  Only all_reduce and broadcast are used, on tensors of the
+model's device.  shard=False keeps every rank a replica.
 """
 from __future__ import annotations
 
@@ -28,13 +36,14 @@ from typing import Callable, Dict, List, Optional, Sequence
 
 import numpy as np
 import torch
+import torch.distributed as dist
 import torch.nn as nn
 
 from . import _lib as L
 from .autoencoder import VQModelInterface
 from .engine import _stream, capture_graphs, frozen_weights, get_plan
 from .ldm import CIN256_V2_CONFIG, UNetModel
-from .scoring import TaylorScorer
+from .scoring import TaylorScorer, _dist_ready
 
 
 class ClassEmbedder(nn.Module):
@@ -255,9 +264,11 @@ class DDIMSampler:
     @torch.no_grad()
     def sample(self, S, batch_size, shape, conditioning=None, callback=None, normals_sequence=None, img_callback=None, quantize_x0=False,
                eta=0., mask=None, x0=None, temperature=1., noise_dropout=0., score_corrector=None, corrector_kwargs=None, verbose=True,
-               x_T=None, log_every_t=100, unconditional_guidance_scale=1., unconditional_conditioning=None, generator=None, **kwargs):
+               x_T=None, log_every_t=100, unconditional_guidance_scale=1., unconditional_conditioning=None, generator=None,
+               step_noise=None, **kwargs):
         """ddim.py:55-104 + ddim_sampling (:106-163): returns (samples, {'x_inter': [...], 'pred_x0': [...]}) with x_T first and the
-        steps whose index % log_every_t == 0 or index == S - 1 after it."""
+        steps whose index % log_every_t == 0 or index == S - 1 after it.  step_noise: the (S, B, C, H, W) per-step noise drawn
+        beforehand, used in place of the S draws on `generator` when eta > 0 (ignored when eta == 0)."""
         unsupported = {"mask / x0": mask is not None or x0 is not None, "quantize_x0": quantize_x0, "score_corrector": score_corrector is not None,
                        "temperature != 1": temperature != 1., "noise_dropout": noise_dropout > 0., "callback / img_callback":
                        callback is not None or img_callback is not None, "ddim_use_original_steps": kwargs.get("ddim_use_original_steps", False),
@@ -291,7 +302,9 @@ class DDIMSampler:
                 if guided:
                     ctx = torch.cat([unconditional_conditioning.reshape(B, 1, -1).to(ctx.device), ctx])
                 plan.load_context(ctx)
-                if run.noise is not None:
+                if run.noise is not None and step_noise is not None:
+                    run.noise.copy_(step_noise.to(dev, torch.float32).reshape(S, B, C_, H, W))
+                elif run.noise is not None:
                     for i in range(S):
                         run.noise[i].copy_(torch.randn((B, C_, H, W), generator=generator, device=gdev, dtype=torch.float32))
                 if run.graph is not None:
@@ -358,6 +371,35 @@ class _nullctx:
         return False
 
 
+def _world_rank(shard: bool):
+    """(world size, rank) of the default process group when `shard` and it has more than one rank; (1, 0) otherwise."""
+    if shard and _dist_ready():
+        return dist.get_world_size(), dist.get_rank()
+    return 1, 0
+
+
+def _round_inputs(draw: Callable[[], Dict[str, torch.Tensor]], spec: Dict[str, tuple], n: int, world: int, rank: int, dev):
+    """The random inputs of this rank's iteration in a round of n <= world consecutive iterations (None when rank >= n).  Rank 0 calls
+    draw() n times, in iteration order, as the single-process loop would, and broadcasts iteration j's draws for rank j; spec gives
+    their {name: (shape, dtype)} for the receiving buffers on `dev`.  Rank 0 keeps its own draws where draw() made them."""
+    mine = None
+    for j in range(n):
+        got = draw() if rank == 0 else None
+        if j > 0:
+            if got is not None:
+                bad = {k: tuple(v.shape) for k, v in got.items() if (tuple(v.shape), v.dtype) != (tuple(spec[k][0]), spec[k][1])}
+                if bad or set(got) != set(spec):
+                    raise RuntimeError(f"drawn inputs {bad or sorted(got)} do not match the broadcast layout {spec}")
+                got = {k: v.to(dev) for k, v in got.items()}
+            else:
+                got = {k: torch.empty(shape, dtype=dtype, device=dev) for k, (shape, dtype) in spec.items()}
+            for k in spec:
+                dist.broadcast(got[k], 0)
+        if j == rank:
+            mine = got
+    return mine
+
+
 PRUNE_LDM_THRESHOLDS = {"taylor": None, "diff-pruning": 0.1, "diff0": 0.0}
 
 
@@ -403,6 +445,11 @@ class LDMPruneScorer:
         self.dev = self.unet.device
         cfg = self.unet.config
         self.shape = (cfg.in_channels, cfg.image_size, cfg.image_size)
+        self.loss_shape = (self.B,) + self.shape         # the latents get_loss_at_t scores (and its noise)
+        if encode_samples:
+            fs = model.first_stage_model
+            f = 2 ** (fs.encoder.num_resolutions - 1)
+            self.loss_shape = (self.B, fs.embed_dim, cfg.image_size // f, cfg.image_size // f)
         self.use_graph = use_graph
         self.sampler = DDIMSampler(model)
         self.sampler.use_graph = use_graph
@@ -410,9 +457,25 @@ class LDMPruneScorer:
         self.g_fwd = self.g_bwd = None
         self.stopped_at: Optional[int] = None
 
-    def _labels(self, class_sampler) -> torch.Tensor:
+    def _draw(self, class_sampler, generator) -> Dict[str, torch.Tensor]:
+        """One iteration's random inputs, in the order the loop consumes them: the class labels (`class_sampler(B)`, or random.sample on
+        the module-level `random`), then on `generator` x_T, the per-step noise (eta > 0 only) and the q_sample noise."""
+        gdev = generator.device if generator is not None else self.dev
         labels = class_sampler(self.B) if class_sampler is not None else random.sample(range(1000), self.B)
-        return torch.as_tensor(labels, dtype=torch.long).to(self.dev)
+        d = {"labels": torch.as_tensor(labels, dtype=torch.long)}
+        d["x_T"] = torch.randn((self.B,) + self.shape, generator=generator, device=gdev, dtype=torch.float32)
+        if self.eta > 0:
+            d["step_noise"] = torch.stack([torch.randn((self.B,) + self.shape, generator=generator, device=gdev, dtype=torch.float32)
+                                           for _ in range(self.S)])
+        d["noise"] = torch.randn(self.loss_shape, generator=generator, device=gdev, dtype=torch.float32)
+        return d
+
+    def _draw_spec(self) -> Dict[str, tuple]:
+        spec = {"labels": ((self.B,), torch.long), "x_T": ((self.B,) + self.shape, torch.float32)}
+        if self.eta > 0:
+            spec["step_noise"] = ((self.S, self.B) + self.shape, torch.float32)
+        spec["noise"] = (self.loss_shape, torch.float32)
+        return spec
 
     def _scorer(self, samples, noise, c) -> TaylorScorer:
         if self.ts is None:
@@ -430,52 +493,96 @@ class LDMPruneScorer:
     def _bwd(self):
         self.ts.plan.run_backward(_stream())
 
+    def _forward(self, t: int, d: Dict[str, torch.Tensor], uc: torch.Tensor) -> torch.Tensor:
+        """Iteration t up to its stop check: context, guided DDIM sample from d's x_T (and step noise), the encoder with encode_samples,
+        then forward + loss at t with d's noise.  Returns the device loss (1,)."""
+        model, B = self.model, self.B
+        c = model.get_learned_conditioning({model.cond_stage_key: d["labels"].to(self.dev)})
+        samples, _ = self.sampler.sample(S=self.S, conditioning=c, batch_size=B, shape=list(self.shape), verbose=False,
+                                         unconditional_guidance_scale=self.scale, unconditional_conditioning=uc, eta=self.eta,
+                                         x_T=d["x_T"], step_noise=d.get("step_noise"))
+        if self.encode_samples:
+            samples = model.encode_first_stage(samples)
+        if tuple(samples.shape) != self.loss_shape:
+            raise RuntimeError(f"the scored latents are {tuple(samples.shape)}, the loss noise was drawn as {self.loss_shape}")
+        ts = self._scorer(samples, d["noise"].to(self.dev), c)
+        p = ts.plan
+        p.check_current()
+        p.attach_grads()
+        p.ensure_packed()
+        p.t_dev.fill_(t)
+        if self.use_graph:
+            if self.g_fwd is None:
+                self.g_fwd, self.g_bwd = capture_graphs(self.dev, self._fwd, self._bwd, restore=(p.grad_arena,))
+            self.g_fwd.replay()
+        else:
+            self._fwd()
+        return ts.loss
+
+    def _backward(self):
+        if self.use_graph:
+            self.g_bwd.replay()
+        else:
+            self._bwd()
+
+    def _grad_arena(self, uc: torch.Tensor) -> torch.Tensor:
+        """The UNet's gradient arena; a rank that ran no iteration (iterations < world) builds the Taylor plan to have one."""
+        if self.ts is None:
+            z = torch.zeros(self.loss_shape, device=self.dev, dtype=torch.float32)
+            self._scorer(z, z, uc)
+        p = self.ts.plan
+        p.check_current()
+        p.attach_grads()
+        return p.grad_arena
+
     def run(self, pruner: str = "taylor", iterations: int = 1000, class_sampler: Optional[Callable[[int], Sequence[int]]] = None,
-            generator: Optional[torch.Generator] = None) -> torch.Tensor:
+            generator: Optional[torch.Generator] = None, shard: bool = True) -> torch.Tensor:
         """The loop of prune_ldm.py:105-131 (test_criterion.py:108-135 with encode_samples) for `pruner` in {taylor, diff-pruning,
         diff0}.  Returns the losses of the iterations that ran (with the stopping one last when the rule stopped the loop, its gradient
-        not accumulated; self.stopped_at is its index)."""
+        not accumulated; self.stopped_at is its index).
+
+        With torch.distributed initialised over W > 1 ranks (and shard=True) the iterations run in rounds of W: rank r runs iteration
+        r0 + r on the inputs rank 0 drew for it, the round's losses are all-reduced (each rank fills its own slot of a W-vector) and every
+        rank replays the stop rule over them in iteration order; an iteration at or after the stopping one skips its backward.  After the
+        last round the gradient arena is all-reduced (SUM) once.  Every rank returns the single-process losses and stopped_at, and holds
+        the single-process gradient up to fp32 summation order.  The gradient already in Parameter.grad counts once, rank 0's: the other
+        ranks zero theirs first."""
         rule = PruneLDMStopRule(pruner)
         model, B = self.model, self.B
-        key = model.cond_stage_key
-        gdev = generator.device if generator is not None else self.dev
+        world, rank = _world_rank(shard and iterations > 0)
         losses: List[float] = []
         self.stopped_at = None
         was_training = self.unet.training
         self.unet.eval()                     # prune_ldm.py:72
         try:
             with torch.no_grad(), frozen_weights(self.unet):
-                uc = model.get_learned_conditioning({key: torch.full((B,), 1000, dtype=torch.long, device=self.dev)})
-                for t in range(iterations):
-                    labels = self._labels(class_sampler)
-                    c = model.get_learned_conditioning({key: labels})
-                    samples, _ = self.sampler.sample(S=self.S, conditioning=c, batch_size=B, shape=list(self.shape), verbose=False,
-                                                     unconditional_guidance_scale=self.scale, unconditional_conditioning=uc, eta=self.eta,
-                                                     generator=generator)
-                    if self.encode_samples:
-                        samples = model.encode_first_stage(samples)
-                    noise = torch.randn(samples.shape, generator=generator, device=gdev, dtype=torch.float32).to(self.dev)
-                    ts = self._scorer(samples, noise, c)
-                    p = ts.plan
-                    p.check_current()
-                    p.attach_grads()
-                    p.ensure_packed()
-                    p.t_dev.fill_(t)
-                    if self.use_graph:
-                        if self.g_fwd is None:
-                            self.g_fwd, self.g_bwd = capture_graphs(self.dev, self._fwd, self._bwd, restore=(p.grad_arena,))
-                        self.g_fwd.replay()
-                    else:
-                        self._fwd()
-                    loss = float(ts.loss.item())
-                    losses.append(loss)
-                    if rule.stop(loss):
-                        self.stopped_at = t
+                uc = model.get_learned_conditioning({model.cond_stage_key: torch.full((B,), 1000, dtype=torch.long, device=self.dev)})
+                if rank > 0:
+                    for p in self.unet.parameters():
+                        if p.grad is not None:
+                            p.grad.zero_()
+                spec = self._draw_spec()
+                for r0 in range(0, iterations, world):
+                    n = min(world, iterations - r0)
+                    d = _round_inputs(lambda: self._draw(class_sampler, generator), spec, n, world, rank, self.dev)
+                    rl = torch.zeros(world, device=self.dev, dtype=torch.float32)
+                    if d is not None:
+                        rl[rank:rank + 1].copy_(self._forward(r0 + rank, d, uc))
+                    if world > 1:
+                        dist.all_reduce(rl, op=dist.ReduceOp.SUM)      # x + 0 is x: every rank reads the losses bit for bit
+                    stop = None
+                    for j, loss in enumerate(rl.tolist()[:n]):
+                        losses.append(loss)
+                        if rule.stop(loss):
+                            stop = j
+                            break
+                    if d is not None and (stop is None or rank < stop):
+                        self._backward()
+                    if stop is not None:
+                        self.stopped_at = r0 + stop
                         break
-                    if self.use_graph:
-                        self.g_bwd.replay()
-                    else:
-                        self._bwd()
+                if world > 1:
+                    dist.all_reduce(self._grad_arena(uc), op=dist.ReduceOp.SUM)
         finally:
             self.unet.train(was_training)
         return torch.tensor(losses, dtype=torch.float32)
@@ -484,13 +591,18 @@ class LDMPruneScorer:
 @torch.no_grad()
 def sample_for_fid(model: LatentDiffusion, classes: Sequence[int] = range(1000), ipc: int = 50, batch_size: int = 50, ddim_steps: int = 250,
                    eta: float = 0., scale: float = 3.0, out_dir: Optional[str] = None, fid_dims: int = 2048, inception=None,
-                   generator: Optional[torch.Generator] = None, decode_batch: int = 8):
+                   generator: Optional[torch.Generator] = None, decode_batch: int = 8, shard: bool = True):
     """sample_for_FID.py:67-100: uc once; then ipc // batch_size rounds over `classes`, each a guided DDIM sample of batch_size latents
     (DDIMSampler, one graph), decode_first_stage in micro-batches of decode_batch (one graph each) and dp_decode_images, which writes
     the bytes tvu.save_image(clamp((x + 1) / 2, 0, 1)) would put in the PNG.  With an Inception model (fid.InceptionV3) the FID moments
     of those bytes accumulate on the device, batch by batch, as fid.calculate_activation_statistics would add the saved files batched
     by batch_size; with out_dir the files `{class_label}_{img_id}.png` are written on the host (img_id counts over the whole run).
-    Returns (mu, sigma, n_files): mu / sigma None without an Inception model, n_files 0 without out_dir."""
+    Returns (mu, sigma, n_files): mu / sigma None without an Inception model, n_files 0 without out_dir.
+
+    With torch.distributed initialised over W > 1 ranks (and shard=True), batch k of the single-process order goes to rank k mod W, on
+    the x_T (and step noise) rank 0 draws for it; each rank writes its own batches' files under their single-process names (out_dir must
+    be one directory all ranks see).  The moments' shift is rank 0's first batch, as in one process; the moments are all-reduced once at
+    the end, and every rank returns the same (mu, sigma, n_files), n_files counting the files of all ranks."""
     if inception is None and out_dir is None:
         raise ValueError("sample_for_fid needs an Inception model, an output directory, or both")
     if not hasattr(model, "first_stage_model"):
@@ -510,19 +622,36 @@ def sample_for_fid(model: LatentDiffusion, classes: Sequence[int] = range(1000),
         from . import fid
         block = fid._block_of(inception, fid_dims)
         mom = fid.Moments(fid_dims)
+    world, rank = _world_rank(shard)
+    batches = [class_label for _ in range(ipc // batch_size) for class_label in classes]
+    gdev = generator.device if generator is not None else dev
+    lat = (batch_size, *shape)
+    spec = {"x_T": (lat, torch.float32)}
+    if eta > 0:
+        spec["step_noise"] = ((ddim_steps,) + lat, torch.float32)
+
+    def draw():      # DDIMSampler.sample's draws: x_T, then one per step when eta > 0
+        d = {"x_T": torch.randn(lat, generator=generator, device=gdev, dtype=torch.float32)}
+        if eta > 0:
+            d["step_noise"] = torch.stack([torch.randn(lat, generator=generator, device=gdev, dtype=torch.float32) for _ in range(ddim_steps)])
+        return d
     u8 = None
-    img_id = n_files = 0
+    n_files = 0
     saved_batch = fs.decode_batch
     fs.decode_batch = decode_batch
     try:
         with model.ema_scope():
             uc = model.get_learned_conditioning({key: torch.tensor(batch_size * [1000]).to(dev)})
-            for _ in range(ipc // batch_size):
-                for class_label in classes:
+            for r0 in range(0, len(batches), world):
+                d = _round_inputs(draw, spec, min(world, len(batches) - r0), world, rank, dev)
+                feat = None
+                if d is not None:
+                    k = r0 + rank
+                    class_label = batches[k]
                     c = model.get_learned_conditioning({key: torch.tensor(batch_size * [class_label]).to(dev)})
                     samples, _ = sampler.sample(S=ddim_steps, conditioning=c, batch_size=batch_size, shape=shape, verbose=False,
                                                 unconditional_guidance_scale=scale, unconditional_conditioning=uc, eta=eta,
-                                                generator=generator)
+                                                x_T=d["x_T"], step_noise=d.get("step_noise"))
                     for s in range(0, batch_size, decode_batch):
                         y = fs.decode_chunk(samples[s:s + decode_batch], inv_scale=inv).plan.y_out
                         if u8 is None:
@@ -534,14 +663,27 @@ def sample_for_fid(model: LatentDiffusion, classes: Sequence[int] = range(1000),
                         plan = inception.plan(batch_size, "u8", u8.shape[1:3])
                         plan.load(u8)
                         plan.run()
-                        mom.add(plan.feat[block])
+                        feat = plan.feat[block]
                     if out_dir is not None:
                         from PIL import Image
-                        for img in u8.cpu().numpy():
-                            Image.fromarray(img).save(os.path.join(out_dir, f"{class_label}_{img_id}.png"))
-                            img_id += 1
+                        for i, img in enumerate(u8.cpu().numpy()):
+                            Image.fromarray(img).save(os.path.join(out_dir, f"{class_label}_{k * batch_size + i}.png"))
                             n_files += 1
+                if mom is not None and world > 1 and r0 == 0:
+                    if rank == 0:
+                        mom.add(feat)          # batch 0 sets the shift, as in one process
+                    mom.share_shift(0)
+                    if rank > 0 and feat is not None:
+                        mom.add(feat)
+                elif feat is not None:
+                    mom.add(feat)
     finally:
         fs.decode_batch = saved_batch
+    if world > 1:
+        if mom is not None:
+            mom.all_reduce()
+        nf = torch.tensor([n_files], dtype=torch.int64, device=dev)
+        dist.all_reduce(nf, op=dist.ReduceOp.SUM)
+        n_files = int(nf.item())
     mu, sigma = mom.finalize() if mom is not None else (None, None)
     return mu, sigma, n_files
