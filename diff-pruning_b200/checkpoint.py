@@ -150,6 +150,7 @@ def allow_module_pickles():
     """torch >= 2.6 defaults torch.load to weights_only=True; the reference stores and reloads WHOLE modules (`torch.save(model)`
     ddpm_prune.py:135 / `torch.load(path)` ddpm_train.py:292, ddpm_sample.py:27).  Allow-list the classes such a pickle contains
     (this package's module classes + the torch.nn leaves + the config containers) so the unchanged `torch.load` call works."""
+    import argparse
     import collections
     import sys
     import torch.nn as nn
@@ -169,6 +170,12 @@ def allow_module_pickles():
     # the weights-only unpickler only fills plain dict / OrderedDict instances (SETITEMS), so the config container of a reference
     # pickle (FrozenDict, an OrderedDict subclass) is materialised as the OrderedDict it is
     cls.append((collections.OrderedDict, "diffusers.configuration_utils.FrozenDict"))
+    # ddpm_exp's pickles (prune.py:281, runners/diffusion_simple.py:270-283) name models.diffusion.*; their `config` is an
+    # argparse.Namespace, and the level / mid / temb containers are plain nn.Module instances
+    from . import ddpm_exp
+    cls += [(getattr(ddpm_exp, n), f"models.diffusion.{n}") for n in ("Model", "ResnetBlock", "AttnBlock", "Downsample", "Upsample")]
+    cls += [ddpm_exp.Model, ddpm_exp.ResnetBlock, ddpm_exp.AttnBlock, ddpm_exp.Downsample, ddpm_exp.Upsample, nn.Module,
+            argparse.Namespace]
     mod = sys.modules.get("diffusers.models.attention_processor")
     if mod is not None and "compat" in (getattr(mod, "__file__", "") or ""):
         cls += [getattr(mod, n) for n in ("AttnProcessor", "AttnProcessor2_0")]

@@ -25,7 +25,7 @@ import torch
 import torch.nn as nn
 
 from . import _lib as L
-from .models import (Attention, Downsample2D, ResnetBlock2D, UNet2DModel, Upsample2D, sinusoidal_frequencies)
+from .models import (Attention, Downsample2D, ResnetBlock2D, UNet2DModel, Upsample2D, ddpm_exp_frequencies, sinusoidal_frequencies)
 
 _byref = C.byref
 Step = Callable[[int], None]
@@ -1046,12 +1046,14 @@ class Plan:
         v.t.zero_()
         return v
 
-    def _time_embedding(self, lin1: nn.Linear, lin2: nn.Linear, flip: bool, shift: float = 0):
+    def _time_embedding(self, lin1: nn.Linear, lin2: nn.Linear, flip: bool, freqs: torch.Tensor):
         """silu_temb = SiLU(lin2(SiLU(lin1(sinusoid(t_dev))))), the per-image input of every resnet's time_emb_proj (embeddings.py:22-62,
-        200-212).  flip: cos | sin halves; shift: the frequency denominator's offset."""
+        200-212).  flip: cos | sin halves; freqs: the host-built fp32 frequency table of the network's embedding (each family rounds its
+        own)."""
         lib, B = self.lib, self.B
         half = lin1.in_features // 2
-        self.freqs = sinusoidal_frequencies(lin1.in_features, shift).to(self.dev)
+        assert freqs.shape == (half,), (tuple(freqs.shape), half)
+        self.freqs = freqs.to(self.dev)
         temb0 = self.new(B, 1, 1, 2 * half)
         l1, s1 = self.new(B, 1, 1, lin1.out_features), self.new(B, 1, 1, lin1.out_features)
         emb = self.new(B, 1, 1, lin2.out_features)
@@ -1116,13 +1118,16 @@ class Plan:
             return self._build_vq_decoder()
         if hasattr(self.model, "quant_conv"):        # VQ first-stage encoder (autoencoder._EncodePath)
             return self._build_vq_encoder()
+        if hasattr(self.model, "temb") and hasattr(self.model, "mid"):     # ddpm_exp's DDIM-codebase Model (ddpm_exp.py)
+            return self._build_ddim_model()
         m = self.model
         H, W = self.H, self.W
         cfg = m.config
         self._setup_param_grads()
         self.t_dev = torch.zeros(self.B, device=self.dev, dtype=torch.int64)
         self.x_in = self._padded(self.B, H, W, cfg.in_channels)
-        self._time_embedding(m.time_embedding.linear_1, m.time_embedding.linear_2, cfg.flip_sin_to_cos, cfg.freq_shift)
+        self._time_embedding(m.time_embedding.linear_1, m.time_embedding.linear_2, cfg.flip_sin_to_cos,
+                             sinusoidal_frequencies(m.time_embedding.linear_1.in_features, cfg.freq_shift))
 
         # ---- skip/concat geometry: every skip lives in the upper channel range of its consumer's concat buffer
         skip_shapes = []
@@ -1346,7 +1351,7 @@ class Plan:
         self.x_in = self._padded(B, H, W, cfg.in_channels)
         self.ctx_in = self._padded(B, 1, 1, cfg.context_dim)
         # exp(-ln(1e4) i / half) (util.py:160-162) in cos | sin order (util.py:164): the DDPM sinusoid with the halves flipped
-        self._time_embedding(m.time_embed[0], m.time_embed[2], flip=True)
+        self._time_embedding(m.time_embed[0], m.time_embed[2], flip=True, freqs=sinusoidal_frequencies(m.time_embed[0].in_features, 0))
 
         def as_resnet(rb):     # ResBlock (openaimodel.py:163-275) in the attribute vocabulary of Plan.resnet()
             sk = rb.skip_connection
@@ -1424,9 +1429,12 @@ class Plan:
 
     # ------------------------------------------------------------------ VQ first-stage decoder (autoencoder.py; cin256-v2 first_stage_config)
     def vq_attention(self, m, x: View, out: View):
-        """AttnBlock (model.py:150-202): GroupNorm(32, eps 1e-6) -> q, k, v as 1x1 convolutions -> softmax(q k^T * c^-0.5) v over the
-        H*W tokens -> 1x1 proj_out ; + x."""
+        """AttnBlock (model.py:150-202; ddpm_exp models/diffusion.py:139-189): GroupNorm(32, eps 1e-6) -> q, k, v as 1x1 convolutions ->
+        softmax(q k^T * c^-0.5) v over the H*W tokens -> 1x1 proj_out ; + x.  c is q's width, as the reference reads it from q.shape at
+        run time: a pruned block scales by its pruned width."""
         N, H, W, Cc = x.N, x.H, x.W, x.C
+        if not m.q.out_channels == m.k.out_channels == m.v.out_channels:
+            raise NotImplementedError(f"AttnBlock with q / k / v widths {m.q.out_channels} / {m.k.out_channels} / {m.v.out_channels}")
         xn = self.new(N, H, W, Cc)
         self.gn(x, m.norm, xn, silu=False)
         convs = (m.q, m.k, m.v)
@@ -1437,21 +1445,41 @@ class Plan:
             for c, t in zip(convs, (q, k, v)):
                 self.conv(xn, c.weight, c.bias, t, pad=0)
         o = self.new(N, H, W, v.C)
-        self._attn_core(q, k, v, o, float(int(Cc) ** -0.5))
+        self._attn_core(q, k, v, o, float(int(m.q.out_channels) ** -0.5))
         self.conv(o, m.proj_out.weight, m.proj_out.bias, out, pad=0, residual=x)
 
-    def _vq_resnet(self, rb, x: View) -> View:
-        """ResnetBlock (model.py:82-141) in the attribute vocabulary of Plan.resnet(), into a new buffer."""
+    def _taming_resnet(self, rb, x: View, out: Optional[View] = None) -> View:
+        """ResnetBlock (model.py:82-141; ddpm_exp models/diffusion.py:76-136, which adds temb_proj) in the attribute vocabulary of
+        Plan.resnet(), into `out` or a new buffer.  The 1x1 nin_shortcut runs when the block was built with in_channels != out_channels:
+        the reference tests those construction-time ints, which pruning leaves as they were."""
         from types import SimpleNamespace as NS
-        y = self.new(x.N, x.H, x.W, rb.out_channels)
-        self.resnet(NS(norm1=rb.norm1, conv1=rb.conv1, time_emb_proj=None, norm2=rb.norm2, dropout=rb.dropout, conv2=rb.conv2,
-                       conv_shortcut=getattr(rb, "nin_shortcut", None), output_scale_factor=1.0), x, y)
+        has_sc = rb.in_channels != rb.out_channels
+        if has_sc and getattr(rb, "use_conv_shortcut", False):
+            raise NotImplementedError("ResnetBlock with a 3x3 conv_shortcut")
+        y = out if out is not None else self.new(x.N, x.H, x.W, rb.conv2.out_channels)
+        self.resnet(NS(norm1=rb.norm1, conv1=rb.conv1, time_emb_proj=getattr(rb, "temb_proj", None), norm2=rb.norm2, dropout=rb.dropout,
+                       conv2=rb.conv2, conv_shortcut=rb.nin_shortcut if has_sc else None, output_scale_factor=1.0), x, y)
         return y
 
-    def _vq_attention_new(self, ab, x: View) -> View:
-        """AttnBlock into a new buffer."""
-        y = self.new(x.N, x.H, x.W, x.C)
+    def _vq_attention_new(self, ab, x: View, out: Optional[View] = None) -> View:
+        """AttnBlock into `out` or a new buffer."""
+        y = out if out is not None else self.new(x.N, x.H, x.W, x.C)
         self.vq_attention(ab, x, y)
+        return y
+
+    def _pad_downsample(self, conv: nn.Conv2d, x: View, out: Optional[View] = None) -> View:
+        """Downsample (model.py:60-79): F.pad(x, (0, 1, 0, 1)) + 3x3 stride-2 convolution without padding, into `out` or a new buffer.  That
+        is the box kernel's stride-2 geometry with pad_t = pad_l = 0: the output grid is the input grid / 2, so the taps that reach the bottom
+        row / right column read past the image and get TMA's zero fill, which is the padding."""
+        assert x.H % 2 == 0 and x.W % 2 == 0, (x.H, x.W)
+        y = out if out is not None else self.new(x.N, x.H // 2, x.W // 2, conv.out_channels)
+        self.conv(x, conv.weight, conv.bias, y, stride=2, pad=0)
+        return y
+
+    def _upsample_conv(self, conv: nn.Conv2d, x: View, out: Optional[View] = None) -> View:
+        """Upsample (model.py:42-57): nearest x2 then a 3x3 convolution, into `out` or a new buffer."""
+        y = out if out is not None else self.new(x.N, 2 * x.H, 2 * x.W, conv.out_channels)
+        self.conv(self._upsample2x(x), conv.weight, conv.bias, y)
         return y
 
     def _build_vq_decoder(self):
@@ -1470,7 +1498,7 @@ class Plan:
         self.conv(self.x_in, m.post_quant_conv.weight, m.post_quant_conv.bias, z, pad=0)
         x = self.new(B, H, W, dec.conv_in.out_channels)
         self.conv(z, dec.conv_in.weight, dec.conv_in.bias, x)
-        resnet, attention = self._vq_resnet, self._vq_attention_new
+        resnet, attention = self._taming_resnet, self._vq_attention_new
         x = resnet(dec.mid.block_2, attention(dec.mid.attn_1, resnet(dec.mid.block_1, x)))
         for i_level in reversed(range(len(dec.up))):
             lvl = dec.up[i_level]
@@ -1479,10 +1507,7 @@ class Plan:
                 if len(lvl.attn) > 0:
                     x = attention(lvl.attn[i_block], x)
             if i_level != 0:
-                u = lvl.upsample.conv
-                y = self.new(x.N, 2 * x.H, 2 * x.W, u.out_channels)
-                self.conv(self._upsample2x(x), u.weight, u.bias, y)
-                x = y
+                x = self._upsample_conv(lvl.upsample.conv, x)
         a = self.new(x.N, x.H, x.W, x.C)
         self.gn(x, dec.norm_out, a, silu=True)
         self.y_out = self._padded(B, x.H, x.W, dec.conv_out.out_channels)
@@ -1492,10 +1517,8 @@ class Plan:
     def _build_vq_encoder(self):
         """VQModelInterface.encode (autoencoder.py:269-272) = quant_conv(Encoder.forward) (model.py:428-460) as a forward-only plan:
         conv_in -> per level, resnets (+ attention) and, below the last level, Downsample -> mid (resnet, attention, resnet) -> GroupNorm
-        + SiLU -> conv_out -> quant_conv.  Downsample's F.pad(x, (0, 1, 0, 1)) + 3x3 stride-2 convolution without padding is the box
-        kernel's stride-2 geometry with pad_t = pad_l = 0: the output grid is the input grid / 2, so the taps that reach the bottom row /
-        right column read past the image and get TMA's zero fill, which is the padding.  B, H, W are the images'; x_in (the images) and
-        y_out (the latents) are padded NHWC buffers."""
+        + SiLU -> conv_out -> quant_conv (Downsample: _pad_downsample).  B, H, W are the images'; x_in (the images) and y_out (the latents)
+        are padded NHWC buffers."""
         if self.need_grad:
             raise NotImplementedError("the VQ encoder plan is forward-only: build it with need_grad=False")
         m = self.model
@@ -1505,18 +1528,14 @@ class Plan:
         self.x_in = self._padded(B, H, W, enc.conv_in.in_channels)
         x = self.new(B, H, W, enc.conv_in.out_channels)
         self.conv(self.x_in, enc.conv_in.weight, enc.conv_in.bias, x)
-        resnet, attention = self._vq_resnet, self._vq_attention_new
+        resnet, attention = self._taming_resnet, self._vq_attention_new
         for lvl in enc.down:
             for i_block, rb in enumerate(lvl.block):
                 x = resnet(rb, x)
                 if len(lvl.attn) > 0:
                     x = attention(lvl.attn[i_block], x)
             if hasattr(lvl, "downsample"):
-                d = lvl.downsample.conv
-                assert x.H % 2 == 0 and x.W % 2 == 0, (x.H, x.W)
-                y = self.new(x.N, x.H // 2, x.W // 2, d.out_channels)
-                self.conv(x, d.weight, d.bias, y, stride=2, pad=0)
-                x = y
+                x = self._pad_downsample(lvl.downsample.conv, x)
         x = resnet(enc.mid.block_2, attention(enc.mid.attn_1, resnet(enc.mid.block_1, x)))
         a = self.new(x.N, x.H, x.W, x.C)
         self.gn(x, enc.norm_out, a, silu=True)
@@ -1524,6 +1543,80 @@ class Plan:
         self.conv(a, enc.conv_out.weight, enc.conv_out.bias, h)
         self.y_out = self._padded(B, x.H, x.W, m.quant_conv.out_channels)
         self.conv(h, m.quant_conv.weight, m.quant_conv.bias, self.y_out, pad=0)
+        self._finalize_build()
+
+    # ------------------------------------------------------------------ ddpm_exp's DDIM-codebase Model (ddpm_exp.py; the paper's CIFAR-10 runs)
+    def _build_ddim_model(self):
+        """Model.forward (ddpm_exp models/diffusion.py:268-300) as a forward-only plan: the sinusoid (sin | cos, ddpm_exp's frequencies)
+        -> temb.dense[0] -> SiLU -> temb.dense[1] -> SiLU once for every ResnetBlock's temb_proj row; conv_in; per level, ResnetBlocks
+        (+ AttnBlocks) and, below the last level, Downsample; mid (block_1, attn_1, block_2); per level from the top, ResnetBlocks over
+        torch.cat([h, hs.pop()]) (+ AttnBlocks) and Upsample; GroupNorm + SiLU -> conv_out.  Every entry of `hs` is written by its producer
+        into the upper channel range of its consumer's concat buffer, as in the DDPM UNet's plan.  B, H, W are the images'; x_in and y_out
+        are padded NHWC buffers, t_dev the (B,) int64 timesteps."""
+        if self.need_grad:
+            raise NotImplementedError("the ddpm_exp Model plan is forward-only: build it with need_grad=False")
+        m = self.model
+        B, H, W = self.B, self.H, self.W
+        d0, d1 = m.temb.dense[0], m.temb.dense[1]
+        if d0.in_features != m.ch or m.ch % 2:
+            raise NotImplementedError(f"time embedding of width {d0.in_features} (ch {m.ch})")
+        if any(not hasattr(lvl.downsample, "conv") for lvl in m.down if hasattr(lvl, "downsample")) or \
+                any(not hasattr(lvl.upsample, "conv") for lvl in m.up if hasattr(lvl, "upsample")):
+            raise NotImplementedError("resamp_with_conv=False (average-pool Downsample / convolution-free Upsample)")
+        self.grad_arena = torch.zeros(0, device=self.dev)
+        self.t_dev = torch.zeros(B, device=self.dev, dtype=torch.int64)
+        self.x_in = self._padded(B, H, W, m.conv_in.in_channels)
+        self._time_embedding(d0, d1, flip=False, freqs=ddpm_exp_frequencies(m.ch))
+        resnet, attention = self._taming_resnet, self._vq_attention_new
+
+        # ---- hs: conv_in, every down block (after its attention), every Downsample; consumed in reverse by the up blocks
+        shapes, hh, ww = [(H, W, m.conv_in.out_channels)], H, W
+        for lvl in m.down:
+            shapes += [(hh, ww, rb.conv2.out_channels) for rb in lvl.block]
+            if hasattr(lvl, "downsample"):
+                hh, ww = hh // 2, ww // 2
+                shapes.append((hh, ww, lvl.downsample.conv.out_channels))
+        ups = [rb for i_level in reversed(range(len(m.up))) for rb in m.up[i_level].block]
+        new_skip = self._skips(shapes, [rb.norm1.num_channels for rb in ups][::-1])
+
+        x = new_skip()
+        self.conv(self.x_in, m.conv_in.weight, m.conv_in.bias, x)
+        hs = [x]
+        for lvl in m.down:
+            for i_block, rb in enumerate(lvl.block):
+                if len(lvl.attn) > 0:
+                    x = attention(lvl.attn[i_block], resnet(rb, x), new_skip())
+                else:
+                    x = resnet(rb, x, new_skip())
+                hs.append(x)
+            if hasattr(lvl, "downsample"):
+                x = self._pad_downsample(lvl.downsample.conv, x, new_skip())
+                hs.append(x)
+
+        # ---- mid: block_2 writes straight into the h half of the first concatenation
+        x = attention(m.mid.attn_1, resnet(m.mid.block_1, x))
+        dest = h_half(hs[-1])
+        assert dest.C == m.mid.block_2.conv2.out_channels and dest.H == x.H, (dest.C, x.C)
+        x = resnet(m.mid.block_2, x, dest)
+
+        # ---- up: the last op of a block writes the h half of the next concatenation, or a new buffer before the output head
+        for i_level in reversed(range(len(m.up))):
+            lvl = m.up[i_level]
+            for i_block, rb in enumerate(lvl.block):
+                cat = cat_of(hs.pop())
+                last = i_block == len(lvl.block) - 1
+                dest = h_half(hs[-1]) if hs and not (last and hasattr(lvl, "upsample")) else None
+                if len(lvl.attn) > 0:
+                    x = attention(lvl.attn[i_block], resnet(rb, cat), dest)
+                else:
+                    x = resnet(rb, cat, dest)
+            if hasattr(lvl, "upsample"):
+                x = self._upsample_conv(lvl.upsample.conv, x, h_half(hs[-1]))
+        assert not hs
+        a = self.new(x.N, x.H, x.W, x.C)
+        self.gn(x, m.norm_out, a, silu=True)
+        self.y_out = self._padded(B, H, W, m.conv_out.out_channels)
+        self.conv(a, m.conv_out.weight, m.conv_out.bias, self.y_out)
         self._finalize_build()
 
     # ------------------------------------------------------------------ execution

@@ -56,6 +56,14 @@ def sinusoidal_frequencies(embedding_dim: int, downscale_freq_shift: float = 1.0
     return torch.exp(exponent)
 
 
+def ddpm_exp_frequencies(embedding_dim: int):
+    """exp(arange(half) * -(ln(1e4) / (half - 1))) as float32 — ddpm_exp models/diffusion.py:16-18 (same op order: the float64 step, then
+    a float32 product and exp; rounds differently in the last bit from sinusoidal_frequencies' float32 quotient)."""
+    half = embedding_dim // 2
+    step = math.log(10000) / (half - 1)
+    return torch.exp(torch.arange(half, dtype=torch.float32) * -step)
+
+
 class Timesteps(nn.Module):
     """embeddings.py:215-229."""
 

@@ -19,6 +19,7 @@ Outputs (all small, committed):
     tests/golden/vq_decoder_tiny.pt  the LDM's VQ first-stage Decoder (small config and VQ-f4 at a 16 x 16 latent) and nearest-code choices
     tests/golden/vq_encoder_tiny.pt  the LDM's VQ first-stage Encoder and VQModelInterface.encode (small config and VQ-f4 at 64 x 64)
     tests/golden/ldm_ddim_tiny.pt  guided DDIM sampling of the tiny LDM by ldm_exp's DDIMSampler, every step, and one get_loss_at_t pass
+    tests/golden/ddpm_exp_tiny.pt  ddpm_exp's Model, generalized_steps and a pruned network on a tiny config (gen_ddpm_exp)
 """
 import argparse
 import hashlib
@@ -27,6 +28,7 @@ import os
 import sys
 import time
 
+import numpy as np
 import torch
 
 HERE = os.path.dirname(os.path.abspath(__file__))
@@ -866,13 +868,111 @@ def gen_vq_encoder():
     print("vq_encoder_tiny.pt", os.path.getsize(os.path.join(OUT, "vq_encoder_tiny.pt")))
 
 
+DDPM_EXP_TINY = {   # ddpm_exp/configs/cifar10.yml at a tiny size: two levels, attention at 8 x 8, 16 x 16 images
+    "data": {"dataset": "CIFAR10", "image_size": 16, "channels": 3, "logit_transform": False, "uniform_dequantization": False,
+             "gaussian_dequantization": False, "random_flip": True, "rescaled": True, "num_workers": 4},
+    "model": {"type": "simple", "in_channels": 3, "out_ch": 3, "ch": 64, "ch_mult": [1, 2], "num_res_blocks": 1, "attn_resolutions": [8],
+              "dropout": 0.1, "var_type": "fixedlarge", "ema_rate": 0.9999, "ema": True, "resamp_with_conv": True},
+    "diffusion": {"beta_schedule": "linear", "beta_start": 0.0001, "beta_end": 0.02, "num_diffusion_timesteps": 1000},
+    "sampling": {"batch_size": 2, "last_only": True},
+}
+
+
+def gen_ddpm_exp():
+    """ddpm_exp's Model and generalized_steps from the UNMODIFIED reference (models/diffusion.py, functions/denoising.py, the vendored
+    torch_pruning) on a tiny config:
+      ddpm_exp_tiny.pt   the seed-0 Model's state-dict keys / shapes / digest, eps_hat at t in {0, 3, 500, 999}, 10-step quad
+                         trajectories at eta 0 and 0.5 (x_T, every step's noise, xs, x0_preds); and a network pruned by the vendored
+                         MagnitudePruner at ratio 0.5 (prune.py:211-281) as the indices of what it kept, with its eps_hat.  The tests pickle
+                         that network under the reference's class names themselves (tests/test_ddpm_exp_host.py)."""
+    import argparse as _ap
+    from models.diffusion import Model as RefModel
+    from oracle import vq_oracle as vo
+    os.chdir("/tmp")
+
+    def ns(d):
+        n = _ap.Namespace()
+        for k, v in d.items():
+            setattr(n, k, ns(v) if isinstance(v, dict) else v)
+        return n
+    cfg = ns(DDPM_EXP_TINY)
+    cfg.device = torch.device("cpu")
+    torch.manual_seed(0)
+    m = RefModel(cfg).eval()
+    d = cfg.diffusion
+    # runners/diffusion.py:44-47 + :76 (get_beta_schedule "linear"; runners/diffusion.py imports dataset packages absent here)
+    betas = torch.from_numpy(np.linspace(d.beta_start, d.beta_end, d.num_diffusion_timesteps, dtype=np.float64)).float()
+    g = torch.Generator().manual_seed(300)
+    x = torch.randn(2, 3, 16, 16, generator=g)
+    out = {"config": DDPM_EXP_TINY, "seed": 0, "sd_keys": list(m.state_dict().keys()),
+           "sd_shapes": [list(v.shape) for v in m.state_dict().values()], "digest": vo.state_dict_digest(m.state_dict()),
+           "x": x, "eps": {}, "traj": {}}
+    with torch.no_grad():
+        for t in (0, 3, 500, 999):
+            out["eps"][t] = m(x, torch.full((2,), float(t))).detach()
+    seq = [int(s) for s in list(np.linspace(0, np.sqrt(1000 * 0.8), 10) ** 2)]
+    for eta in (0.0, 0.5):
+        torch.manual_seed(7)
+        x_T = torch.randn(2, 3, 16, 16)
+        noises = []
+        xs, x0s = ref_shim.cpu_generalized_steps(noises)(x_T, seq, m, betas, eta=eta)
+        out["traj"][eta] = {"seq": seq, "x_T": x_T, "noise": torch.stack(noises), "xs": torch.stack(xs), "x0s": torch.stack(x0s)}
+        print("ddpm_exp traj", eta, float(xs[-1].abs().max()))
+    # the pruned network: seed 0 with distinct 1-D parameters (xo.distinct_vectors), pruned by the reference pruner; the fixture keeps the
+    # indices of the surviving rows / columns of every parameter, from which xo.prune_like rebuilds it
+    from oracle import ddpm_exp_oracle as xo
+    torch.manual_seed(0)
+    m = xo.distinct_vectors(RefModel(cfg).eval())
+    orig = {k: v.detach().clone() for k, v in m.state_dict().items()}
+    example = {"x": torch.randn(1, 3, 16, 16), "t": torch.ones(1)}
+    pruner = tp.pruner.MagnitudePruner(m, example, importance=tp.importance.MagnitudeImportance(), iterative_steps=1, channel_groups={},
+                                       ch_sparsity=0.5, ignored_layers=[m.conv_out], root_module_types=[torch.nn.Conv2d, torch.nn.Linear])
+    for grp in pruner.step(interactive=True):
+        grp.prune()
+    m.zero_grad()
+    del pruner
+
+    def where(src, vals):        # position of every value of `vals` in the distinct-valued vector `src`
+        pos = {float(v): i for i, v in enumerate(src.tolist())}
+        assert len(pos) == src.numel()
+        return [pos[float(v)] for v in vals.tolist()]
+    keep = {}
+    pruned = {k: v for k, v in m.state_dict().items() if v.shape != orig[k].shape}
+    for k, v in pruned.items():               # vectors first: every conv / linear keeps the rows its bias keeps
+        if v.dim() == 1:
+            keep[k] = (where(orig[k], v), None)
+    for k, v in pruned.items():
+        if v.dim() == 1:
+            continue
+        rows = keep.get(k[:-len("weight")] + "bias", (None,))[0]
+        o = orig[k] if rows is None else orig[k][torch.tensor(rows)]
+        cols = None
+        if v.shape[1] != o.shape[1]:          # the kept input columns, matched as whole columns of the kept rows
+            oc, vc = o.transpose(0, 1).reshape(o.shape[1], -1), v.transpose(0, 1).reshape(v.shape[1], -1)
+            cols = [int((oc == c).all(1).nonzero()[0, 0]) for c in vc]
+        keep[k] = (rows, cols)
+    from diff_pruning_b200 import ddpm_exp as de
+    torch.manual_seed(0)
+    rebuilt = xo.prune_like(xo.distinct_vectors(de.Model(DDPM_EXP_TINY).eval()), keep)
+    assert all(torch.equal(a, b) for a, b in zip(rebuilt.state_dict().values(), m.state_dict().values()))
+    assert list(rebuilt.state_dict()) == list(m.state_dict())
+    with torch.no_grad():
+        out["pruned_eps"] = {t: m(x, torch.full((2,), float(t))).detach() for t in (0, 500)}
+    out["pruned_keep"] = keep
+    out["pruned_shapes"] = {k: list(v.shape) for k, v in m.state_dict().items()}
+    out["pruned_shortcuts"] = {n: mod.in_channels != mod.out_channels for n, mod in m.named_modules() if hasattr(mod, "temb_proj")}
+    torch.save(out, os.path.join(OUT, "ddpm_exp_tiny.pt"))
+    print("ddpm_exp_tiny.pt", os.path.getsize(os.path.join(OUT, "ddpm_exp_tiny.pt")))
+    print("pruned widths", sorted({v[0] for k, v in out["pruned_shapes"].items() if k.endswith("weight")}))
+
+
 if __name__ == "__main__":
     ap = argparse.ArgumentParser()
     ap.add_argument("--skip-cfg1", action="store_true")
     ap.add_argument("--only", default=None)
     a = ap.parse_args()
     torch.set_num_threads(os.cpu_count())
-    jobs = {"vq_encoder": gen_vq_encoder, "vq_decoder": gen_vq_decoder, "ssim": gen_ssim, "fid": gen_fid,"ldm_tiny": gen_ldm_tiny, "ldm_ddim": gen_ldm_ddim, "exp_importance": gen_exp_importance, "ref_pickle": gen_ref_pickle, "lsun_struct": gen_lsun_struct, "lr": gen_lr, "ckpt": gen_ckpt, "ddim": gen_ddim, "tiny": gen_tiny, "blocks": gen_blocks, "finetune": gen_finetune, "cifar_fwd": gen_cifar_fwd,
+    jobs = {"ddpm_exp": gen_ddpm_exp, "vq_encoder": gen_vq_encoder, "vq_decoder": gen_vq_decoder, "ssim": gen_ssim, "fid": gen_fid,"ldm_tiny": gen_ldm_tiny, "ldm_ddim": gen_ldm_ddim, "exp_importance": gen_exp_importance, "ref_pickle": gen_ref_pickle, "lsun_struct": gen_lsun_struct, "lr": gen_lr, "ckpt": gen_ckpt, "ddim": gen_ddim, "tiny": gen_tiny, "blocks": gen_blocks, "finetune": gen_finetune, "cifar_fwd": gen_cifar_fwd,
             "cfg1_s3": gen_cfg1_s3, "cfg3_s3": gen_cfg3_s3, "cfg1": gen_cfg1}
     for name, fn in jobs.items():
         if a.only and name != a.only:

@@ -91,3 +91,29 @@ def cpu_ddim_sampler():
         def register_buffer(self, name, attr):
             setattr(self, name, attr)
     return CpuDDIMSampler
+
+
+def cpu_generalized_steps(record=None):
+    """ddpm_exp's generalized_steps (functions/denoising.py:10-33) on the CPU: the unmodified function, run with `Tensor.to('cuda')`
+    (denoising.py:20 hard-codes it) redirected to the CPU.  record: a list that receives every torch.randn_like draw (the step noise)."""
+    from functions.denoising import generalized_steps
+
+    def run(*a, **kw):
+        to, randn_like = torch.Tensor.to, torch.randn_like
+
+        def to_cpu(self, *args, **kwargs):
+            if args and args[0] == "cuda":
+                args = ("cpu",) + args[1:]
+            return to(self, *args, **kwargs)
+
+        def draw(*args, **kwargs):
+            n = randn_like(*args, **kwargs)
+            if record is not None:
+                record.append(n.clone())
+            return n
+        torch.Tensor.to, torch.randn_like = to_cpu, draw
+        try:
+            return generalized_steps(*a, **kw)
+        finally:
+            torch.Tensor.to, torch.randn_like = to, randn_like
+    return run
