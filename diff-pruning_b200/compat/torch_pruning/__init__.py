@@ -122,6 +122,7 @@ class MagnitudePruner:
                 if imp is None:
                     continue
                 grp.idxs = _sc.select_pruning_idxs(imp, g["ch_groups"], n_pruned)
+                grp.imp, grp.ch_groups, grp.n_pruned = imp, g["ch_groups"], n_pruned     # what the selection was made from
                 yield grp
         if interactive:
             return gen()

@@ -1,10 +1,14 @@
-"""ddpm_exp's FID sampling loop (the DDIM codebase that produced the paper's CIFAR-10 results) on the engine, forward only.
+"""ddpm_exp's FID sampling loop and prune.py's Taylor loop (the DDIM codebase that produced the paper's CIFAR-10 results) on the engine.
 
 Model          — ddpm_exp/models/diffusion.py:192-300: module tree, names and construction order of the reference, so
                  `torch.manual_seed(s); Model(cfg)` draws the reference's parameters and the state dicts match key for key.  The leaves are
                  nn.Conv2d / nn.Linear / nn.GroupNorm; AttnBlock, Downsample and Upsample are the VQ first stage's (autoencoder.py), which
                  the reference copied from the same source.  Model.forward(x, t) runs the planned sm_90a engine (Plan._build_ddim_model)
-                 on CUDA under torch.no_grad(); with grad enabled or on the CPU it raises.
+                 on CUDA; with grad enabled it is one autograd node whose backward fills Parameter.grad.  On the CPU it raises outside
+                 models.trace_mode(), under which the modules run their torch forward (models/diffusion.py:113-136, 268-300).
+noise_estimation_loss, taylor_loop, OursStopRule
+               — functions/losses.py:4-15 and prune.py:236-258: the Taylor-importance loop over 1000 timesteps as graph replays
+                 (TaylorScorer.forward_loss / backward), with the `--pruner ours` stop rule.
 EMAHelper      — models/ema.py: register / state_dict / load_state_dict / ema, the shadow a list.
 load_model     — runners/diffusion.py:100-195: a pickled pruned Model, a pickled [Model, ..., ema_shadow] list, a ckpt.pth list
                  [Module | state_dict, optimizer, epoch, step, (ema)], or a plain state dict from a local path.
@@ -30,10 +34,13 @@ from typing import Optional
 import numpy as np
 import torch
 import torch.nn as nn
+import torch.nn.functional as F
 
 from . import _lib as L
 from .autoencoder import AttnBlock, Downsample, Normalize, Upsample
 from .engine import _stream, capture_graphs, frozen_weights, get_plan, unet_apply
+from .models import ddpm_exp_frequencies
+from .models import tracing as trace_mode_active
 
 
 CIFAR10_CONFIG = {   # ddpm_exp/configs/cifar10.yml
@@ -79,6 +86,27 @@ class ResnetBlock(nn.Module):
         self.conv2 = nn.Conv2d(out_channels, out_channels, kernel_size=3, stride=1, padding=1)
         if self.in_channels != self.out_channels:
             self.nin_shortcut = nn.Conv2d(in_channels, out_channels, kernel_size=1, stride=1, padding=0)
+
+    def forward(self, x, temb):
+        """models/diffusion.py:113-136 in torch: the module-by-module forward of models.trace_mode() (the pruning tracer and the op
+        counter walk it); Model.forward runs the engine plan otherwise."""
+        h = self.conv1(_silu(self.norm1(x)))
+        h = h + self.temb_proj(_silu(temb))[:, :, None, None]
+        h = self.conv2(self.dropout(_silu(self.norm2(h))))
+        if self.in_channels != self.out_channels:
+            x = self.nin_shortcut(x)
+        return x + h
+
+
+def _silu(x):
+    return x * torch.sigmoid(x)
+
+
+def _timestep_embedding(t: torch.Tensor, dim: int) -> torch.Tensor:
+    """get_timestep_embedding (models/diffusion.py:6-24): sin | cos of t * ddpm_exp's frequencies."""
+    emb = t.float()[:, None] * ddpm_exp_frequencies(dim).to(t.device)[None, :]
+    emb = torch.cat([torch.sin(emb), torch.cos(emb)], dim=1)
+    return F.pad(emb, (0, 1, 0, 0)) if dim % 2 == 1 else emb
 
 
 class Model(nn.Module):
@@ -159,12 +187,13 @@ class Model(nn.Module):
         return {k: v for k, v in self.__dict__.items() if not k.startswith("_dpb200")}
 
     def forward(self, x, t):
-        """models/diffusion.py:268-300 on the engine.  t: (B,) timesteps, integer-valued (generalized_steps passes them as float)."""
-        if torch.is_grad_enabled():
-            raise RuntimeError("diff_pruning_b200: the ddpm_exp Model runs forward only; call it under torch.no_grad() "
-                               "(its training, Taylor and finetune paths are not on the engine)")
+        """models/diffusion.py:268-300 on the engine.  t: (B,) timesteps, integer-valued (generalized_steps passes them as float).  With
+        grad enabled the plan records its backward and `loss.backward()` accumulates into Parameter.grad (prune.py:236-258); x gets no
+        gradient.  Under models.trace_mode() the modules run in torch, on any device."""
+        if trace_mode_active():
+            return self._torch_forward(x, t)
         if x.device.type != "cuda":
-            raise RuntimeError("diff_pruning_b200: the ddpm_exp Model runs on a CUDA device (no CPU fallback)")
+            raise RuntimeError("diff_pruning_b200: the ddpm_exp Model runs on a CUDA device (no CPU fallback outside models.trace_mode())")
         if self.training and any(m.p > 0 for m in self.modules() if isinstance(m, nn.Dropout)):
             raise RuntimeError("diff_pruning_b200: the ddpm_exp Model plan is an evaluation plan (dropout off): call model.eval()")
         assert x.shape[2] == x.shape[3] == self.resolution
@@ -172,6 +201,39 @@ class Model(nn.Module):
         if t.is_floating_point() and not torch.equal(t, t.trunc()):
             raise ValueError("diff_pruning_b200: the ddpm_exp Model plan takes integer-valued timesteps")
         return unet_apply(self, x, t)
+
+    def _torch_forward(self, x, t):
+        assert x.shape[2] == x.shape[3] == self.resolution
+        temb = self.temb.dense[1](_silu(self.temb.dense[0](_timestep_embedding(torch.as_tensor(t, device=x.device), self.ch))))
+        hs = [self.conv_in(x)]
+        for i_level in range(self.num_resolutions):
+            for i_block in range(self.num_res_blocks):
+                h = self.down[i_level].block[i_block](hs[-1], temb)
+                if len(self.down[i_level].attn) > 0:
+                    h = self.down[i_level].attn[i_block](h)
+                hs.append(h)
+            if i_level != self.num_resolutions - 1:
+                hs.append(self.down[i_level].downsample(hs[-1]))
+        h = self.mid.block_2(self.mid.attn_1(self.mid.block_1(hs[-1], temb)), temb)
+        for i_level in reversed(range(self.num_resolutions)):
+            for i_block in range(self.num_res_blocks + 1):
+                h = self.up[i_level].block[i_block](torch.cat([h, hs.pop()], dim=1), temb)
+                if len(self.up[i_level].attn) > 0:
+                    h = self.up[i_level].attn[i_block](h)
+            if i_level != 0:
+                h = self.up[i_level].upsample(h)
+        return self.conv_out(_silu(self.norm_out(h)))
+
+
+def noise_estimation_loss(model, x0: torch.Tensor, t: torch.Tensor, e: torch.Tensor, b: torch.Tensor, keepdim: bool = False):
+    """functions/losses.py:4-15 for autograd callers: a = (1 - b).cumprod(0)[t], x = x0 sqrt(a) + e sqrt(1 - a), then
+    ||e - model(x, t)||^2 summed over C, H, W per image, and averaged over the batch unless keepdim."""
+    a = (1 - b).cumprod(dim=0).index_select(0, t).view(-1, 1, 1, 1)
+    x = x0 * a.sqrt() + e * (1.0 - a).sqrt()
+    output = model(x, t.float())
+    if keepdim:
+        return (e - output).square().sum(dim=(1, 2, 3))
+    return (e - output).square().sum(dim=(1, 2, 3)).mean(dim=0)
 
 
 class EMAHelper:
@@ -245,6 +307,133 @@ def load_model(config, path: Optional[str] = None, pruned: Optional[str] = None,
     else:
         raise ValueError("load_model needs a checkpoint path or a pruned model file")
     return model.eval()
+
+
+# ------------------------------------------------------------------------------------------------------------------- Taylor loop
+class OursStopRule:
+    """prune.py:248-253 (`--pruner ours`): max_loss starts at 0 and takes the loss when the loss exceeds it; the loop breaks when
+    loss < max_loss * thr, an fp32 product as on the reference's 0-dim fp32 tensors, BEFORE loss.backward(): the stopping step's gradient
+    is not accumulated.  A NaN loss neither raises max_loss nor stops."""
+
+    def __init__(self, thr: float):
+        self.thr = np.float32(thr)
+        self.max_loss = np.float32(0.0)
+
+    def stop(self, loss: float) -> bool:
+        l32 = np.float32(loss)
+        if l32 > self.max_loss:
+            self.max_loss = l32
+        return bool(l32 < self.max_loss * self.thr)
+
+
+STOPPING_PRUNERS = ("ours",)
+TAYLOR_LOOP_PRUNERS = ("taylor", "first_order_taylor", "second_order_taylor", "abs_taylor", "fisher", "ours")   # prune.py:236
+
+
+def taylor_loop(model: Model, x: torch.Tensor, e: torch.Tensor, betas: torch.Tensor, pruner: str = "taylor", thr: float = 0.01,
+                n_steps: int = 1000, use_graph: bool = True):
+    """The loop of prune.py:236-258 on the engine: for step_k = 0 .. n_steps - 1, noise_estimation_loss(model, x, t = step_k for every
+    image, e, betas) and its backward, the gradients accumulating into Parameter.grad from zero (model.zero_grad() first).  x (the data
+    batch after data_transform) and e are (B, C, H, W) fp32 on a CUDA device, fixed for every step; betas the fp32 schedule, whose alphas
+    table is (1 - b).cumprod(0) on the betas' device, as the loss computes it.
+
+    Every step is one forward + loss graph replay and one backward graph replay (TaylorScorer.forward_loss / backward).  With
+    pruner "ours" the host reads every step's loss and OursStopRule decides before the backward; the other pruners never stop and the
+    losses stay on the device until the end.  Returns (losses of the steps that ran, the stopping one last, as a CPU fp32 tensor;
+    the index of the stopping step or None)."""
+    from .scoring import TaylorScorer
+    if pruner not in TAYLOR_LOOP_PRUNERS:
+        raise ValueError(f"prune.py runs its Taylor loop for {TAYLOR_LOOP_PRUNERS}, not {pruner!r}")
+    if n_steps > betas.shape[0]:      # the reference's index_select fails past the table; the device gather would read past it
+        raise ValueError(f"n_steps {n_steps} exceeds the {betas.shape[0]} timesteps of the schedule")
+    if x.device.type != "cuda":
+        raise RuntimeError("diff_pruning_b200: the ddpm_exp Taylor loop runs on a CUDA device (no CPU fallback)")
+    acp = (1 - betas).cumprod(dim=0).to(x.device)
+    model.zero_grad()
+    ts = TaylorScorer(model, x, e, alphas_cumprod=acp, use_graph=use_graph, reduction="sum_mean")
+    rule = OursStopRule(thr) if pruner in STOPPING_PRUNERS else None
+    losses = torch.zeros(n_steps, device=x.device, dtype=torch.float32)
+    stopped_at = None
+    for k in range(n_steps):
+        loss = ts.forward_loss(k)
+        losses[k:k + 1].copy_(loss)
+        if rule is not None and rule.stop(float(loss.item())):
+            stopped_at = k
+            break
+        ts.backward()
+    n = n_steps if stopped_at is None else stopped_at + 1
+    return losses[:n].cpu(), stopped_at
+
+
+PRUNERS = ("taylor", "random", "magnitude", "reinit", "first_order_taylor", "second_order_taylor", "abs_taylor", "fisher", "ours")
+
+
+def _importance(pruner: str):
+    """prune.py:191-208: the vendored torch_pruning importance of each `--pruner`, on the engine's device reductions."""
+    from .compat import torch_pruning as tp
+    if pruner in ("taylor", "ours"):
+        return tp.importance.TaylorImportance(variant="vendored")         # the vendored sum_k (w dw)^2
+    if pruner in ("first_order_taylor", "second_order_taylor"):
+        return tp.importance.FullTaylorImportance(order=1 if pruner == "first_order_taylor" else 2)
+    if pruner == "abs_taylor":
+        return tp.importance.AbsTaylorImportance()
+    if pruner == "fisher":
+        return tp.importance.FisherImportance()
+    if pruner == "magnitude":
+        return tp.importance.MagnitudeImportance()
+    return tp.importance.RandomImportance()                                # random, reinit
+
+
+def prune(model: Model, config, x: torch.Tensor, pruner: str, pruning_ratio: float, thr: float = 0.01, timesteps: int = 1000,
+          skip_type: str = "uniform", eta: float = 0.0, n_steps: int = 1000, use_graph: bool = True, preview: bool = True):
+    """prune.py:179-291 for a Model on a CUDA device (in place), x the loaded batch in [0, 1] (B, C, S, S).  In the reference's order:
+    the example input (torch.randn on the CPU generator, then moved, as prune.py:190 draws it), MagnitudePruner over the Model's groups
+    (conv_out ignored), the MACs / parameters before, the preview noise (sampling.batch_size images on the device generator), then for the
+    Taylor criteria data_transform(x) (`rescaled`: 2 x - 1), e = randn_like(x) and taylor_loop; the interactive pruner step, the
+    `reinit` re-initialisation, the MACs / parameters after and the preview sample (sample_image from the preview noise; preview=False
+    skips it).  Returns a SimpleNamespace: model, macs (before, after), params (before, after), losses, stopped_at, groups (root,
+    channels, ch_groups, n_pruned, imp, idxs of every pruned group, in order) and samples.  torch.save(model) writes what prune.py:281
+    writes; load_model(config, pruned=...) reads it back."""
+    from .compat import torch_pruning as tp
+    config = dict2namespace(config)
+    if pruner not in PRUNERS:
+        raise ValueError(f"pruner must be one of {PRUNERS}, got {pruner!r}")
+    if getattr(config.data, "logit_transform", False) or not getattr(config.data, "rescaled", True) or hasattr(config, "image_mean") or \
+            getattr(config.data, "uniform_dequantization", False) or getattr(config.data, "gaussian_dequantization", False):
+        raise NotImplementedError("data_transform other than `rescaled` (2 x - 1)")
+    dev = next(model.parameters()).device
+    if dev.type != "cuda":
+        raise RuntimeError("diff_pruning_b200: ddpm_exp.prune runs on a CUDA device (no CPU fallback)")
+    model.eval()
+    S = config.data.image_size
+    example = {"x": torch.randn(1, 3, S, S).to(dev), "t": torch.ones(1).to(dev)}
+    imp = _importance(pruner)
+    mp = tp.pruner.MagnitudePruner(model, example, importance=imp, iterative_steps=1, channel_groups={}, ch_sparsity=pruning_ratio,
+                                   ignored_layers=[model.conv_out], root_module_types=[nn.Conv2d, nn.Linear])
+    base_macs, base_params = tp.utils.count_ops_and_params(model, example)
+    noise = torch.randn(config.sampling.batch_size, config.data.channels, S, S, device=dev)
+    betas = beta_schedule(config).to(dev)
+    losses, stopped_at = torch.zeros(0), None
+    if pruner in TAYLOR_LOOP_PRUNERS:
+        x = 2 * x.to(dev, torch.float32) - 1.0
+        e = torch.randn_like(x)
+        losses, stopped_at = taylor_loop(model, x, e, betas, pruner, thr, n_steps, use_graph)
+    groups = []
+    for g in mp.step(interactive=True):
+        groups.append({"root": g.root, "channels": g.channels, "ch_groups": g.ch_groups, "n_pruned": g.n_pruned, "imp": g.imp,
+                       "idxs": list(g.idxs)})
+        g.prune()
+    if pruner == "reinit":
+        def reset_parameters(_):          # prune.py:270-274: the function resets every module of the model on each call of apply
+            for m in model.modules():
+                if hasattr(m, "reset_parameters"):
+                    m.reset_parameters()
+        model.apply(reset_parameters)
+    macs, params = tp.utils.count_ops_and_params(model, example)
+    samples = sample_image(noise, model, betas, timesteps, skip_type, eta) if preview else None
+    return SimpleNamespace(model=model, macs=(base_macs, macs), params=(base_params, params), losses=losses, stopped_at=stopped_at,
+                           groups=groups, samples=samples)
+
 
 
 # ------------------------------------------------------------------------------------------------------------------- sampling

@@ -1436,7 +1436,9 @@ class Plan:
         if not m.q.out_channels == m.k.out_channels == m.v.out_channels:
             raise NotImplementedError(f"AttnBlock with q / k / v widths {m.q.out_channels} / {m.k.out_channels} / {m.v.out_channels}")
         xn = self.new(N, H, W, Cc)
-        self.gn(x, m.norm, xn, silu=False)
+        g = self.gn(x, m.norm, xn, silu=False)
+        if self.need_grad:      # x.grad = GroupNorm backward of xn.grad + out.grad (the residual)
+            self.gn_bwd(g, x, m.norm, lambda xn=xn: self.gradof(xn).ptr, self.gradof(xn).ld, add2=self.gradof(out))
         convs = (m.q, m.k, m.v)
         if self.qkv_fusable(xn, convs):
             q, k, v = self.conv_qkv(xn, convs)
@@ -1547,14 +1549,13 @@ class Plan:
 
     # ------------------------------------------------------------------ ddpm_exp's DDIM-codebase Model (ddpm_exp.py; the paper's CIFAR-10 runs)
     def _build_ddim_model(self):
-        """Model.forward (ddpm_exp models/diffusion.py:268-300) as a forward-only plan: the sinusoid (sin | cos, ddpm_exp's frequencies)
+        """Model.forward (ddpm_exp models/diffusion.py:268-300) as a plan: the sinusoid (sin | cos, ddpm_exp's frequencies)
         -> temb.dense[0] -> SiLU -> temb.dense[1] -> SiLU once for every ResnetBlock's temb_proj row; conv_in; per level, ResnetBlocks
         (+ AttnBlocks) and, below the last level, Downsample; mid (block_1, attn_1, block_2); per level from the top, ResnetBlocks over
         torch.cat([h, hs.pop()]) (+ AttnBlocks) and Upsample; GroupNorm + SiLU -> conv_out.  Every entry of `hs` is written by its producer
         into the upper channel range of its consumer's concat buffer, as in the DDPM UNet's plan.  B, H, W are the images'; x_in and y_out
-        are padded NHWC buffers, t_dev the (B,) int64 timesteps."""
-        if self.need_grad:
-            raise NotImplementedError("the ddpm_exp Model plan is forward-only: build it with need_grad=False")
+        are padded NHWC buffers, t_dev the (B,) int64 timesteps.  With need_grad every block records its backward as in the DDPM UNet's
+        plan (prune.py's Taylor loop): the gradients go to the parameter arena, the input gets none."""
         m = self.model
         B, H, W = self.B, self.H, self.W
         d0, d1 = m.temb.dense[0], m.temb.dense[1]
@@ -1563,7 +1564,10 @@ class Plan:
         if any(not hasattr(lvl.downsample, "conv") for lvl in m.down if hasattr(lvl, "downsample")) or \
                 any(not hasattr(lvl.upsample, "conv") for lvl in m.up if hasattr(lvl, "upsample")):
             raise NotImplementedError("resamp_with_conv=False (average-pool Downsample / convolution-free Upsample)")
-        self.grad_arena = torch.zeros(0, device=self.dev)
+        if self.need_grad:
+            self._setup_param_grads()
+        else:
+            self.grad_arena = torch.zeros(0, device=self.dev)
         self.t_dev = torch.zeros(B, device=self.dev, dtype=torch.int64)
         self.x_in = self._padded(B, H, W, m.conv_in.in_channels)
         self._time_embedding(d0, d1, flip=False, freqs=ddpm_exp_frequencies(m.ch))
@@ -1580,7 +1584,7 @@ class Plan:
         new_skip = self._skips(shapes, [rb.norm1.num_channels for rb in ups][::-1])
 
         x = new_skip()
-        self.conv(self.x_in, m.conv_in.weight, m.conv_in.bias, x)
+        self.conv(self.x_in, m.conv_in.weight, m.conv_in.bias, x, need_dx=False)
         hs = [x]
         for lvl in m.down:
             for i_block, rb in enumerate(lvl.block):
@@ -1613,10 +1617,7 @@ class Plan:
             if hasattr(lvl, "upsample"):
                 x = self._upsample_conv(lvl.upsample.conv, x, h_half(hs[-1]))
         assert not hs
-        a = self.new(x.N, x.H, x.W, x.C)
-        self.gn(x, m.norm_out, a, silu=True)
-        self.y_out = self._padded(B, H, W, m.conv_out.out_channels)
-        self.conv(a, m.conv_out.weight, m.conv_out.bias, self.y_out)
+        self._out_head(x, m.norm_out, m.conv_out)
         self._finalize_build()
 
     # ------------------------------------------------------------------ execution

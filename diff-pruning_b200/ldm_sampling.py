@@ -454,7 +454,6 @@ class LDMPruneScorer:
         self.sampler = DDIMSampler(model)
         self.sampler.use_graph = use_graph
         self.ts: Optional[TaylorScorer] = None
-        self.g_fwd = self.g_bwd = None
         self.stopped_at: Optional[int] = None
 
     def _draw(self, class_sampler, generator) -> Dict[str, torch.Tensor]:
@@ -479,19 +478,22 @@ class LDMPruneScorer:
 
     def _scorer(self, samples, noise, c) -> TaylorScorer:
         if self.ts is None:
-            self.ts = TaylorScorer(self.unet, samples, noise, alphas_cumprod=self.model.alphas_cumprod, use_graph=False, context=c)
+            self.ts = TaylorScorer(self.unet, samples, noise, alphas_cumprod=self.model.alphas_cumprod, use_graph=self.use_graph,
+                                   context=c)
         else:
             self.ts.clean.copy_(samples)
             self.ts.noise.copy_(noise)
             self.ts.plan.load_context(c)
         return self.ts
 
-    def _fwd(self):
-        self.ts._refresh_noise()
-        self.ts._forward_loss()
+    @property
+    def g_fwd(self):
+        """The forward + loss graph of the Taylor pass (TaylorScorer.forward_loss), None before the first iteration."""
+        return self.ts.g_fwd if self.ts is not None else None
 
-    def _bwd(self):
-        self.ts.plan.run_backward(_stream())
+    @property
+    def g_bwd(self):
+        return self.ts.g_bwd if self.ts is not None else None
 
     def _forward(self, t: int, d: Dict[str, torch.Tensor], uc: torch.Tensor) -> torch.Tensor:
         """Iteration t up to its stop check: context, guided DDIM sample from d's x_T (and step noise), the encoder with encode_samples,
@@ -505,25 +507,10 @@ class LDMPruneScorer:
             samples = model.encode_first_stage(samples)
         if tuple(samples.shape) != self.loss_shape:
             raise RuntimeError(f"the scored latents are {tuple(samples.shape)}, the loss noise was drawn as {self.loss_shape}")
-        ts = self._scorer(samples, d["noise"].to(self.dev), c)
-        p = ts.plan
-        p.check_current()
-        p.attach_grads()
-        p.ensure_packed()
-        p.t_dev.fill_(t)
-        if self.use_graph:
-            if self.g_fwd is None:
-                self.g_fwd, self.g_bwd = capture_graphs(self.dev, self._fwd, self._bwd, restore=(p.grad_arena,))
-            self.g_fwd.replay()
-        else:
-            self._fwd()
-        return ts.loss
+        return self._scorer(samples, d["noise"].to(self.dev), c).forward_loss(t)
 
     def _backward(self):
-        if self.use_graph:
-            self.g_bwd.replay()
-        else:
-            self._bwd()
+        self.ts.backward()
 
     def _grad_arena(self, uc: torch.Tensor) -> torch.Tensor:
         """The UNet's gradient arena; a rank that ran no iteration (iterations < world) builds the Taylor plan to have one."""

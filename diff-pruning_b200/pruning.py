@@ -133,12 +133,20 @@ def traced_module_order(model) -> List[str]:
     fn2mod = {}
     hooks = [m.register_forward_hook(lambda mod, i, o: fn2mod.__setitem__(o.grad_fn, mod)) for m in leaves]
     cfg = model.config
-    size = cfg.sample_size if isinstance(cfg.sample_size, int) else 32
     p0 = next(model.parameters())
     was_training = model.training
     model.eval()
     with torch.enable_grad(), trace_mode():
-        out = model(torch.randn(1, cfg.in_channels, size, size, device=p0.device), torch.ones(1, dtype=torch.long, device=p0.device)).sample
+        if _is_ddim_model(model):       # prune.py:190: example_inputs {'x': randn(1, 3, S, S), 't': torch.ones(1)}
+            # the trace input comes from a generator of its own: the reference's tracer draws nothing, and RandomImportance's draws
+            # later in prune.py must see the global generator where the reference leaves it
+            size = cfg.data.image_size
+            x = torch.randn(1, model.in_channels, size, size, generator=torch.Generator().manual_seed(0)).to(p0.device)
+            out = model(x, torch.ones(1, device=p0.device))
+        else:
+            size = cfg.sample_size if isinstance(cfg.sample_size, int) else 32
+            out = model(torch.randn(1, cfg.in_channels, size, size, device=p0.device),
+                        torch.ones(1, dtype=torch.long, device=p0.device)).sample
     for h in hooks:
         h.remove()
     model.train(was_training)
@@ -165,12 +173,19 @@ def traced_module_order(model) -> List[str]:
     return order
 
 
+def _is_ddim_model(model) -> bool:
+    """ddpm_exp's DDIM-codebase Model (ddpm_exp.py), which the planner recognises the same way."""
+    return hasattr(model, "temb") and hasattr(model, "mid")
+
+
 def build_groups(model, ignored_layers: Sequence[nn.Module] = (), module_order: Sequence[str] = None) -> List[dict]:
-    """Current pruning groups of a UNet2DModel: [{root, ch_groups, channels, items: [(layer_name, kind, idxs)]}] in the
-    reference's group order.  `idxs` map the root's channel positions to each member's own indices (concat offsets);
+    """Current pruning groups of a UNet2DModel or of ddpm_exp's Model: [{root, ch_groups, channels, items: [(layer_name, kind, idxs)]}]
+    in the reference's group order.  `idxs` map the root's channel positions to each member's own indices (concat offsets);
     a member fed twice by the same space carries the merged map (len = 2*channels) like the reference."""
-    from .models import Attention, ResnetBlock2D, UNet2DModel
-    assert isinstance(model, UNet2DModel)
+    from types import SimpleNamespace as NS
+    from .models import UNet2DModel
+    ddim = _is_ddim_model(model)
+    assert ddim or isinstance(model, UNet2DModel)
     names = {m: n for n, m in model.named_modules()}
     if module_order is None:
         module_order = traced_module_order(model)
@@ -189,7 +204,7 @@ def build_groups(model, ignored_layers: Sequence[nn.Module] = (), module_order: 
             sp.add(s, (kind, layer, off, n))
             off += n
 
-    def resnet(m: ResnetBlock2D, segs, temb_space):
+    def resnet(m, segs, temb_space):        # ResnetBlock2D, or a ddpm_exp ResnetBlock in its attribute vocabulary
         consume(m.norm1, segs, "gn")
         consume(m.conv1, segs)
         a = produce(m.conv1)
@@ -206,7 +221,7 @@ def build_groups(model, ignored_layers: Sequence[nn.Module] = (), module_order: 
             b = produce(m.conv2, segs[0][0])
         return [(b, m.conv2.out_channels)]
 
-    def attention(m: Attention, segs):
+    def attention(m, segs):                 # Attention, or a ddpm_exp AttnBlock (1x1 convolutions) in its attribute vocabulary
         assert len(segs) == 1
         s, n = segs[0]
         consume(m.group_norm, segs, "gn")
@@ -215,10 +230,19 @@ def build_groups(model, ignored_layers: Sequence[nn.Module] = (), module_order: 
         v = produce(m.to_q)
         produce(m.to_k, v)
         produce(m.to_v, v)
-        consume(m.to_out[0], [(v, m.to_q.out_features)])
+        consume(m.to_out[0], [(v, m.to_q.weight.shape[0])])
         produce(m.to_out[0], s)
         return segs
 
+    if ddim:
+        _ddim_spaces(model, produce, consume, resnet, attention, NS)
+    else:
+        _unet2d_spaces(model, produce, consume, resnet, attention)
+    sp.add(sp.new(), ("out", model.conv_out, 0, model.conv_out.out_channels))
+    return _groups_of(sp, names, order, ignored)
+
+
+def _unet2d_spaces(model, produce, consume, resnet, attention):
     te = model.time_embedding
     t1 = produce(te.linear_1)
     consume(te.linear_2, [(t1, te.linear_1.out_features)])
@@ -252,8 +276,51 @@ def build_groups(model, ignored_layers: Sequence[nn.Module] = (), module_order: 
             x = [(produce(conv), conv.out_channels)]
     consume(model.conv_norm_out, x, "gn")
     consume(model.conv_out, x)
-    sp.add(sp.new(), ("out", model.conv_out, 0, model.conv_out.out_channels))
 
+
+def _ddim_spaces(model, produce, consume, resnet, attention, NS):
+    """Model.forward (ddpm_exp models/diffusion.py:268-300): temb.dense, conv_in, the down levels with their hs entries, mid, the up levels
+    over torch.cat([h, hs.pop()]), norm_out and conv_out.  A ResnetBlock applies nin_shortcut when it was built with in_channels !=
+    out_channels; q / k / v / proj_out are 1x1 convolutions."""
+    def rb(m, segs, t):
+        return resnet(NS(norm1=m.norm1, conv1=m.conv1, time_emb_proj=m.temb_proj, norm2=m.norm2, conv2=m.conv2,
+                         conv_shortcut=m.nin_shortcut if m.in_channels != m.out_channels else None), segs, t)
+
+    def ab(m, segs):
+        return attention(NS(group_norm=m.norm, to_q=m.q, to_k=m.k, to_v=m.v, to_out=[m.proj_out]), segs)
+    d0, d1 = model.temb.dense
+    t1 = produce(d0)
+    consume(d1, [(t1, d0.out_features)])
+    t2 = produce(d1)
+    x = [(produce(model.conv_in), model.conv_in.out_channels)]
+    hs = [x]
+    for lvl in model.down:
+        for i, m in enumerate(lvl.block):
+            x = rb(m, x, t2)
+            if len(lvl.attn) > 0:
+                x = ab(lvl.attn[i], x)
+            hs.append(x)
+        if hasattr(lvl, "downsample"):
+            conv = lvl.downsample.conv
+            consume(conv, x)
+            x = [(produce(conv), conv.out_channels)]
+            hs.append(x)
+    x = rb(model.mid.block_2, ab(model.mid.attn_1, rb(model.mid.block_1, x, t2)), t2)
+    for i_level in reversed(range(len(model.up))):
+        lvl = model.up[i_level]
+        for i, m in enumerate(lvl.block):
+            x = rb(m, x + hs.pop(), t2)
+            if len(lvl.attn) > 0:
+                x = ab(lvl.attn[i], x)
+        if hasattr(lvl, "upsample"):
+            conv = lvl.upsample.conv
+            consume(conv, x)
+            x = [(produce(conv), conv.out_channels)]
+    consume(model.norm_out, x, "gn")
+    consume(model.conv_out, x)
+
+
+def _groups_of(sp, names, order, ignored) -> List[dict]:
     groups = []
     for root_space, members in sp.members.items():
         prods = [mem for mem in members if mem[0] == "out"]

@@ -35,7 +35,12 @@ class TaylorScorer:
 
     def __init__(self, model: UNet2DModel, clean_images: torch.Tensor, noise: torch.Tensor,
                  num_train_timesteps: int = 1000, alphas_cumprod: Optional[torch.Tensor] = None, use_graph: bool = True,
-                 fused_scores: bool = False, context: Optional[torch.Tensor] = None):
+                 fused_scores: bool = False, context: Optional[torch.Tensor] = None, reduction: str = "mean"):
+        """reduction: the loss the gradient is taken of.  "mean": F.mse_loss's mean over every element (ddpm_prune.py:101).
+        "sum_mean": the squared error summed over C, H, W per image, then averaged over the batch (ddpm_exp functions/losses.py:4-15,
+        the loss of prune.py's loop)."""
+        if reduction not in ("mean", "sum_mean"):
+            raise ValueError(f"reduction must be 'mean' or 'sum_mean', got {reduction!r}")
         assert clean_images.is_cuda and clean_images.shape == noise.shape and clean_images.dtype == torch.float32
         self.lib = L.load()
         self.model = model
@@ -66,7 +71,10 @@ class TaylorScorer:
         self.loss = torch.zeros(1, device=self.dev, dtype=torch.float32)
         self.use_graph = use_graph
         self.graph: Optional[torch.cuda.CUDAGraph] = None
-        self.loss_scale, self.grad_scale = 1.0 / n, 2.0 / n   # F.mse_loss mean reduction, ddpm_prune.py:101
+        self.g_fwd: Optional[torch.cuda.CUDAGraph] = None     # forward_loss / backward: the pass split at the loss
+        self.g_bwd: Optional[torch.cuda.CUDAGraph] = None
+        d = n if reduction == "mean" else B
+        self.loss_scale, self.grad_scale = 1.0 / d, 2.0 / d
         self._refresh_noise()
         self.plan.attach_grads()
         self.plan.ensure_packed()
@@ -88,6 +96,38 @@ class TaylorScorer:
     def _body(self):
         self._forward_loss()
         self.plan.run_backward(_stream())
+
+    def _fwd_body(self):
+        self._refresh_noise()
+        self._forward_loss()
+
+    def _bwd_body(self):
+        self.plan.run_backward(_stream())
+
+    def forward_loss(self, t: int) -> torch.Tensor:
+        """The first half of a pass, for loops that read the loss before they decide on the backward (a stop rule): the current noise
+        to NHWC, add_noise, forward and loss at timestep t, as one graph replay (use_graph) or the eager launches.  Returns the device
+        loss (1,); the gradient d loss / d output waits in the plan for backward()."""
+        p = self.plan
+        p.check_current()
+        p.attach_grads()
+        p.ensure_packed()
+        p.t_dev.fill_(int(t))
+        if self.use_graph:
+            if self.g_fwd is None:
+                self.g_fwd, self.g_bwd = capture_graphs(self.dev, self._fwd_body, self._bwd_body,
+                                                        restore=(p.grad_arena, p.score_arena if p.fused_scores else None))
+            self.g_fwd.replay()
+        else:
+            self._fwd_body()
+        return self.loss
+
+    def backward(self):
+        """The second half: the backward of the last forward_loss, accumulating into Parameter.grad."""
+        if self.use_graph:
+            self.g_bwd.replay()
+        else:
+            self._bwd_body()
 
     def signed_scores(self) -> Dict[str, Tuple[torch.Tensor, torch.Tensor]]:
         """{weight name: (out-channel, in-channel) sum_t sum_k W*dW_t} accumulated by the fused reduce (fused_scores=True)."""

@@ -20,6 +20,8 @@ Outputs (all small, committed):
     tests/golden/vq_encoder_tiny.pt  the LDM's VQ first-stage Encoder and VQModelInterface.encode (small config and VQ-f4 at 64 x 64)
     tests/golden/ldm_ddim_tiny.pt  guided DDIM sampling of the tiny LDM by ldm_exp's DDIMSampler, every step, and one get_loss_at_t pass
     tests/golden/ddpm_exp_tiny.pt  ddpm_exp's Model, generalized_steps and a pruned network on a tiny config (gen_ddpm_exp)
+    tests/golden/ddpm_exp_loop_tiny.pt  prune.py's 1000-step Taylor loop on the same config, and an `ours` run that stops (gen_ddpm_exp_loop)
+    tests/golden/ddpm_exp_prune_tiny.pt prune.py's pruner step for every criterion on that config, and the CIFAR-10 group structure
 """
 import argparse
 import hashlib
@@ -966,13 +968,199 @@ def gen_ddpm_exp():
     print("pruned widths", sorted({v[0] for k, v in out["pruned_shapes"].items() if k.endswith("weight")}))
 
 
+def gen_ddpm_exp_loop(B=4, n_steps=1000):
+    """prune.py's Taylor loop (prune.py:236-258) from the UNMODIFIED reference (models/diffusion.py Model, functions/losses.py
+    noise_estimation_loss) on DDPM_EXP_TINY, seed 0, on the CPU:
+      ddpm_exp_loop_tiny.pt  x (data_transform of a seeded [0, 1] batch, `rescaled`: 2 x - 1) and e; the loss of every one of the 1000
+                             steps with each step's backward accumulating (every pruner but `ours`), and the fingerprints of every
+                             Parameter.grad after the loop; an `ours` run at a thr chosen to stop mid-loop: thr, the stop index, the
+                             margins of the losses / running-max ratios from thr, and the gradient fingerprints at the stop."""
+    import argparse as _ap
+    from models.diffusion import Model as RefModel
+    from functions.losses import noise_estimation_loss
+    os.chdir("/tmp")
+
+    def ns(d):
+        n = _ap.Namespace()
+        for k, v in d.items():
+            setattr(n, k, ns(v) if isinstance(v, dict) else v)
+        return n
+    cfg = ns(DDPM_EXP_TINY)
+    cfg.device = torch.device("cpu")
+    d = cfg.diffusion
+    b = torch.from_numpy(np.linspace(d.beta_start, d.beta_end, d.num_diffusion_timesteps, dtype=np.float64)).float()
+    g = torch.Generator().manual_seed(401)
+    x01 = torch.rand(B, 3, 16, 16, generator=g)
+    x = 2 * x01 - 1.0                              # datasets/__init__.py data_transform, config.data.rescaled
+    e = torch.randn(B, 3, 16, 16, generator=g)
+
+    def loop(thr=None):
+        torch.manual_seed(0)
+        model = RefModel(cfg).eval()
+        model.zero_grad()
+        losses, max_loss, stop = [], 0, None
+        for step_k in range(n_steps):            # prune.py:246-258, `args.pruner == 'ours'` when thr is given
+            t = torch.ones(B, dtype=torch.long) * step_k
+            loss = noise_estimation_loss(model, x, t, e, b)
+            losses.append(float(loss))
+            if thr is not None:
+                if loss > max_loss:
+                    max_loss = loss
+                if loss < max_loss * thr:
+                    stop = step_k
+                    break
+            loss.backward()
+        return model, losses, stop
+
+    t0 = time.time()
+    model, losses, _ = loop()
+    print("ddpm_exp loop", n_steps, "steps", f"{time.time() - t0:.1f} s", losses[0], losses[-1])
+    out = {"config": DDPM_EXP_TINY, "seed": 0, "x01": x01, "x": x, "e": e, "losses": torch.tensor(losses),
+           "grad_fp": {k: fp(p.grad) for k, p in model.named_parameters()}}
+    # thr for `ours`: with r_k = loss_k / max(loss_0..k) (fp32 as the reference computes it), the smallest ratio m before step K, the
+    # first later step s whose ratio is below m, and thr = (m + r_s) / 2 -- the loop stops at s, every ratio at least (m - r_s) / 2 from thr
+    l32 = torch.tensor(losses, dtype=torch.float32)
+    r = (l32 / torch.cummax(l32, 0).values).tolist()
+    best = None
+    for K in range(50, 700, 10):
+        m = min(r[:K])
+        s = next((k for k in range(K, n_steps) if r[k] < m), None)
+        if s is not None and (best is None or m - r[s] > best[0]):
+            best = (m - r[s], K, m, s)
+    _, K, m, s = best
+    thr = (m + r[s]) / 2
+    model, ours_losses, stop = loop(thr)
+    assert stop == s, (stop, s)
+    out["ours"] = {"thr": thr, "stop": stop, "losses": torch.tensor(ours_losses), "margin": (m - r[s]) / 2,
+                   "grad_fp": {k: fp(p.grad) for k, p in model.named_parameters()}}
+    print("ddpm_exp ours: thr", thr, "stop", stop, "margin", (m - r[s]) / 2)
+    torch.save(out, os.path.join(OUT, "ddpm_exp_loop_tiny.pt"))
+    print("ddpm_exp_loop_tiny.pt", os.path.getsize(os.path.join(OUT, "ddpm_exp_loop_tiny.pt")))
+
+
+def gen_ddpm_exp_prune(B=4, ratio=0.3):
+    """prune.py:179-291 from the UNMODIFIED reference (models/diffusion.py, functions/losses.py, the vendored torch_pruning's
+    MagnitudePruner, importances and count_ops_and_params) on DDPM_EXP_TINY, seed 0, on the CPU, for every `--pruner`:
+      ddpm_exp_prune_tiny.pt  per criterion: the interactive group records (root, channels, ch_groups, n_pruned, items, imp, selected
+                              indices), MACs and parameters before and after, the pruned state dict's shapes and digest and its eps_hat at
+                              t = 500 on x; and the CIFAR-10 config's group structure (root, channels, ch_groups, items) from one batch-1
+                              trace.  Draws follow prune.py with the device draws (preview noise, e) on a generator of their own, as they
+                              land on the CUDA generator there: torch.manual_seed(0), the example input, then for the Taylor criteria the
+                              1000-step loop of ddpm_exp_loop_tiny.pt's x and e (`ours` at its thr)."""
+    import argparse as _ap
+    import copy
+    from models.diffusion import Model as RefModel
+    from functions.losses import noise_estimation_loss
+    from oracle import vq_oracle as vo
+    os.chdir("/tmp")
+
+    def ns(d):
+        n = _ap.Namespace()
+        for k, v in d.items():
+            setattr(n, k, ns(v) if isinstance(v, dict) else v)
+        return n
+    loop = torch.load(os.path.join(OUT, "ddpm_exp_loop_tiny.pt"), weights_only=False)
+    x, e = loop["x"], loop["e"]
+    cfg = ns(DDPM_EXP_TINY)
+    cfg.device = torch.device("cpu")
+    d = cfg.diffusion
+    b = torch.from_numpy(np.linspace(d.beta_start, d.beta_end, d.num_diffusion_timesteps, dtype=np.float64)).float()
+    S = cfg.data.image_size
+
+    def taylor_grads(thr=None):
+        torch.manual_seed(0)
+        model = RefModel(cfg).eval()
+        model.zero_grad()
+        max_loss = 0
+        for step_k in range(1000):
+            loss = noise_estimation_loss(model, x, torch.ones(B, dtype=torch.long) * step_k, e, b)
+            if thr is not None:
+                if loss > max_loss:
+                    max_loss = loss
+                if loss < max_loss * thr:
+                    break
+            loss.backward()
+        return {k: p.grad.clone() for k, p in model.named_parameters()}
+    grads = {"taylor": taylor_grads(), "ours": taylor_grads(loop["ours"]["thr"])}
+    imps = {"taylor": lambda: tp.importance.TaylorImportance(), "ours": lambda: tp.importance.TaylorImportance(),
+            "first_order_taylor": lambda: tp.importance.FullTaylorImportance(order=1),
+            "second_order_taylor": lambda: tp.importance.FullTaylorImportance(order=2),
+            "abs_taylor": lambda: tp.importance.AbsTaylorImportance(), "fisher": lambda: tp.importance.FisherImportance(),
+            "magnitude": lambda: tp.importance.MagnitudeImportance(), "random": lambda: tp.importance.RandomImportance(),
+            "reinit": lambda: tp.importance.RandomImportance()}
+    out = {"config": DDPM_EXP_TINY, "seed": 0, "ratio": ratio, "x": x, "e": e, "thr": loop["ours"]["thr"], "criteria": {}}
+    for pruner_name, make in imps.items():
+        torch.manual_seed(0)
+        m = RefModel(cfg).eval()
+        names = {mod: n for n, mod in m.named_modules()}
+        example = {"x": torch.randn(1, 3, S, S), "t": torch.ones(1)}
+        imp = make()
+        pruner = tp.pruner.MagnitudePruner(m, example, importance=imp, iterative_steps=1, channel_groups={}, ch_sparsity=ratio,
+                                           ignored_layers=[m.conv_out], root_module_types=[torch.nn.Conv2d, torch.nn.Linear])
+        base = tp.utils.count_ops_and_params(m, example)
+        if pruner_name in grads or pruner_name in ("first_order_taylor", "second_order_taylor", "abs_taylor", "fisher"):
+            gsrc = grads["ours" if pruner_name == "ours" else "taylor"]
+            for k, p in m.named_parameters():
+                p.grad = gsrc[k].clone()
+        groups = []
+        for g in pruner.step(interactive=True):
+            module, fn = g[0][0].target.module, g[0][0].handler
+            cur = pruner.DG.get_out_channels(module)
+            full = pruner.DG.get_pruning_group(module, fn, list(range(cur)))
+            n_pruned = cur - int(pruner.layer_init_out_ch[module] * (1 - pruner.get_target_sparsity(module)))
+            chg = int(pruner.get_channel_groups(full))
+            # the group's importance as the pruner scored it (not re-drawn for the random criteria: that would move the CPU generator)
+            score = None if pruner_name in ("random", "reinit") else imp(full, ch_groups=chg).clone()
+            groups.append({"root": names[module], "channels": int(cur), "ch_groups": chg, "n_pruned": int(n_pruned),
+                           "items": describe_group_c(full, names), "imp": score, "idxs": [int(i) for i in g[0][1]]})
+            g.prune()
+        if pruner_name == "reinit":
+            def reset_parameters(model):
+                for mm in m.modules():
+                    if hasattr(mm, "reset_parameters"):
+                        mm.reset_parameters()
+            m.apply(reset_parameters)
+        after = tp.utils.count_ops_and_params(m, example)
+        sd = m.state_dict()
+        with torch.no_grad():
+            eps = m(x[:2], torch.full((2,), 500.0)).detach()
+        out["criteria"][pruner_name] = {"groups": groups, "base": base, "pruned": after, "shapes": {k: list(v.shape) for k, v in sd.items()},
+                                        "digest": vo.state_dict_digest(sd), "eps_t500": eps}
+        print("ddpm_exp prune", pruner_name, base, after, len(groups), flush=True)
+    # the group structure of the unpruned tiny and CIFAR-10 networks from one batch-1 trace: the interactive step without prune()
+    def structure(c, hw):
+        torch.manual_seed(0)
+        cc = ns(c)
+        cc.device = torch.device("cpu")
+        m = RefModel(cc).eval()
+        names = {mod: n for n, mod in m.named_modules()}
+        example = {"x": torch.randn(1, 3, hw, hw), "t": torch.ones(1)}
+        pruner = tp.pruner.MagnitudePruner(m, example, importance=tp.importance.MagnitudeImportance(), iterative_steps=1,
+                                           channel_groups={}, ch_sparsity=0.3, ignored_layers=[m.conv_out],
+                                           root_module_types=[torch.nn.Conv2d, torch.nn.Linear])
+        res = []
+        for g in pruner.step(interactive=True):
+            module, fn = g[0][0].target.module, g[0][0].handler
+            cur = pruner.DG.get_out_channels(module)
+            full = pruner.DG.get_pruning_group(module, fn, list(range(cur)))
+            res.append({"root": names[module], "channels": int(cur), "ch_groups": int(pruner.get_channel_groups(full)),
+                        "items": describe_group_c(full, names)})
+        return res, tp.utils.count_ops_and_params(m, example)
+    from diff_pruning_b200.ddpm_exp import CIFAR10_CONFIG
+    out["tiny_groups"], _ = structure(DDPM_EXP_TINY, S)
+    out["cifar_groups"], out["cifar_counts"] = structure(CIFAR10_CONFIG, 32)
+    cg = out["cifar_groups"]
+    torch.save(out, os.path.join(OUT, "ddpm_exp_prune_tiny.pt"))
+    print("ddpm_exp_prune_tiny.pt", os.path.getsize(os.path.join(OUT, "ddpm_exp_prune_tiny.pt")), len(cg), "CIFAR-10 groups")
+
+
 if __name__ == "__main__":
     ap = argparse.ArgumentParser()
     ap.add_argument("--skip-cfg1", action="store_true")
     ap.add_argument("--only", default=None)
     a = ap.parse_args()
     torch.set_num_threads(os.cpu_count())
-    jobs = {"ddpm_exp": gen_ddpm_exp, "vq_encoder": gen_vq_encoder, "vq_decoder": gen_vq_decoder, "ssim": gen_ssim, "fid": gen_fid,"ldm_tiny": gen_ldm_tiny, "ldm_ddim": gen_ldm_ddim, "exp_importance": gen_exp_importance, "ref_pickle": gen_ref_pickle, "lsun_struct": gen_lsun_struct, "lr": gen_lr, "ckpt": gen_ckpt, "ddim": gen_ddim, "tiny": gen_tiny, "blocks": gen_blocks, "finetune": gen_finetune, "cifar_fwd": gen_cifar_fwd,
+    jobs = {"ddpm_exp_prune": gen_ddpm_exp_prune, "ddpm_exp_loop": gen_ddpm_exp_loop, "ddpm_exp": gen_ddpm_exp, "vq_encoder": gen_vq_encoder, "vq_decoder": gen_vq_decoder, "ssim": gen_ssim, "fid": gen_fid,"ldm_tiny": gen_ldm_tiny, "ldm_ddim": gen_ldm_ddim, "exp_importance": gen_exp_importance, "ref_pickle": gen_ref_pickle, "lsun_struct": gen_lsun_struct, "lr": gen_lr, "ckpt": gen_ckpt, "ddim": gen_ddim, "tiny": gen_tiny, "blocks": gen_blocks, "finetune": gen_finetune, "cifar_fwd": gen_cifar_fwd,
             "cfg1_s3": gen_cfg1_s3, "cfg3_s3": gen_cfg3_s3, "cfg1": gen_cfg1}
     for name, fn in jobs.items():
         if a.only and name != a.only:
